@@ -133,7 +133,8 @@ const char *rda_version(void);
  * Front end: the steps either side of the solve, batched and stateless (SURVEY.md §8 f1-f3).
  * All pointers are DEVICE pointers; every call only enqueues one kernel on cuda_stream.
  * ------------------------------------------------------------------------------------------ */
-#define RDA_MAX_SHAPES 64     /* raw obstacles per instance handed to rda_convert_obstacles */
+#define RDA_MAX_SHAPES 64     /* raw obstacles per instance handed to rda_convert_obstacles (only there) */
+#define RDA_MAX_WORLD_SLOTS 256 /* N accepted by rda_convert_world_obstacles (worlds: any size) */
 
 /* MPC.pre_process (mpc.py:251-291) with closest_point :338-353, inter_point :355-383,
  * range_cir_seg :385-423, wraptopi :431-438 and motion_predict_model_* :293-336, for B
@@ -164,6 +165,26 @@ int rda_convert_obstacles(int B, int M, int N, int T, int E, float dt, int time_
                           const float *shape_xy, const float *shape_radius, const float *shape_vel,
                           const int32_t *shape_count, float *obs_A, float *obs_b, int32_t *obs_kind,
                           int32_t *obs_count, void *cuda_stream);
+
+/* The same conversion when robots share obstacle WORLDS of any size, as MPC.control receives
+ * everything the simulator knows: convert_rda_obstacle (mpc.py:189-218) over the robot's whole
+ * world, stable-sorted by rda_obs_distance when order != 0, then assign_obstacle_parameter
+ * (rda_solver.py:483-526) keeps the first N and pads by repeating the last.  Per robot the
+ * result equals rda_convert_obstacles given that robot's world as its list, without the
+ * RDA_MAX_SHAPES limit and without a private copy per robot.
+ *   shape_kind, shape_nv, shape_xy, shape_radius, shape_vel: ONE flat list of S shapes, per-shape
+ *   layout as rda_convert_obstacles ([S], [S], [S][RDA_MAX_EDGE][2], [S], [S][2]);
+ *   world_start [W+1]: world w is shapes [world_start[w], world_start[w+1]);
+ *   robot_world [B]: the world of each robot (NULL: all in world 0; outside [0, W): no obstacles);
+ *   state [B][3]: sort key origin (may be NULL when order = 0).
+ * N <= RDA_MAX_WORLD_SLOTS.  obs_count [B] receives the world size (len(obstacle_list)); a robot
+ * whose world is empty gets all-zero slots.  Out: obs_A, obs_b, obs_kind, obs_count exactly as
+ * rda_inputs expects them.                                                                 */
+int rda_convert_world_obstacles(int B, int W, int N, int T, int E, float dt, int time_varying, int order,
+                                const float *state, const int32_t *world_start, const int32_t *robot_world,
+                                const int32_t *shape_kind, const int32_t *shape_nv, const float *shape_xy,
+                                const float *shape_radius, const float *shape_vel, float *obs_A,
+                                float *obs_b, int32_t *obs_kind, int32_t *obs_count, void *cuda_stream);
 
 /* Arrive rule of MPC.control (mpc.py:170-185, single gear): instances whose near_index >=
  * P - goal_index_threshold get u_opt = 0 and arrive = 1; cur_vel (may be NULL) receives the

@@ -47,8 +47,9 @@ EXPORTS = ['rda_create', 'rda_destroy', 'rda_set_tunables', 'rda_get_tunables', 
            'rda_cold_start', 'rda_solve', 'rda_begin', 'rda_step_su', 'rda_step_lammuz', 'rda_finish',
            'rda_get_buffer', 'rda_copy_buffer', 'rda_last_launch_count', 'rda_version',
            'rda_pre_process', 'rda_convert_obstacles', 'rda_post_process', 'rda_motion_predict',
-           'rda_pre_process_curves', 'rda_post_process_gear']
+           'rda_pre_process_curves', 'rda_post_process_gear', 'rda_convert_world_obstacles']
 MAX_SHAPES = 64
+MAX_WORLD_SLOTS = 256
 
 _lib = None
 
@@ -83,6 +84,7 @@ def load():
     i, f = C.c_int, C.c_float
     lib.rda_pre_process.argtypes = [i, i, i, f, f, vp, vp, vp, vp, i, vp, f, i, vp, vp, vp, vp]
     lib.rda_convert_obstacles.argtypes = [i, i, i, i, i, f, i, i] + [vp] * 12
+    lib.rda_convert_world_obstacles.argtypes = [i, i, i, i, i, f, i, i] + [vp] * 13
     lib.rda_post_process.argtypes = [i, i, i, i, vp, vp, vp, vp, vp]
     lib.rda_pre_process_curves.argtypes = [i, i, i, f, f, vp, vp, vp, vp, i, vp, vp, vp, f, i, vp, vp, vp, vp]
     lib.rda_post_process_gear.argtypes = [i, i, i, vp, i, vp, vp, vp, vp, vp, vp]

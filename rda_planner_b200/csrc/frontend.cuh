@@ -185,6 +185,9 @@ RDA_HD void obstacle_rows(int kind, int nv, const float* xy, double radius, doub
   }
 }
 
+// the order of the stable sort by key: ties go to the lower list index
+RDA_HD bool obstacle_before(double ka, int ia, double kb, int ib) { return ka < kb || (ka == kb && ia < ib); }
+
 // Which raw shape fills slot n of an instance (stable ascending order of the keys when `order`,
 // otherwise list order; slots beyond the list repeat its last element): returns -1 for an empty list.
 // keys[] is scratch of at least `count` doubles already filled by the caller when order != 0.

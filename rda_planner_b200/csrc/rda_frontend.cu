@@ -90,6 +90,118 @@ k_convert_obstacles(int B, int M, int N, int T, int E, float dt, int time_varyin
   }
 }
 
+// Shared worlds: one CTA per robot scans its world in tiles of kWorldTile shapes, one key per thread, and keeps the
+// N first (key, index) pairs of the stable order sorted in shared memory.  Only shapes that beat the current N-th
+// pair are compacted; they are ranked among themselves and merged with the kept list by binary search (every
+// element's new position is its rank in its own list plus its rank in the other).  A tile's indices all exceed the
+// kept ones, so once N are kept a shape beats the N-th only with a strictly smaller key: after the first tiles a
+// shape costs its key and nothing else.  The world is read by every robot in it and stays in L2.
+constexpr int kWorldTile = 256;
+
+__device__ __forceinline__ int world_rank(const double* key, const int* idx, int n, double k, int i) {
+  int lo = 0, hi = n;                                  // number of pairs in the sorted list before (k, i)
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (obstacle_before(key[mid], idx[mid], k, i)) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+__global__ void __launch_bounds__(kWorldTile)
+k_convert_world_obstacles(int B, int W, int N, int T, int E, float dt, int time_varying, int order, const float* state,
+                          const int* world_start, const int* robot_world, const int* shape_kind, const int* shape_nv,
+                          const float* shape_xy, const float* shape_radius, const float* shape_vel, float* obs_A,
+                          float* obs_b, int* obs_kind, int* obs_count) {
+  // dynamic shared memory (order != 0): kept keys [2][N], candidate keys [2][tile], kept indices [2][N],
+  // candidate indices [2][tile]; the kept list is double-buffered, candidates are gathered then sorted
+  extern __shared__ double sh[];
+  __shared__ int n_cand[3];                            // candidate counter of tile k is n_cand[k % 3]
+  const int b = blockIdx.x;
+  if (b >= B) return;
+  const int tid = threadIdx.x;
+  const int w = robot_world ? robot_world[b] : 0;
+  int first = 0, count = 0;
+  if (w >= 0 && w < W) {
+    first = world_start[w];
+    count = world_start[w + 1] - first;
+    if (count < 0) count = 0;
+  }
+  int cur = 0;
+  int* kept_idx = nullptr;
+  if (order && count > 0) {
+    double* kkey = sh;                                 // [2][N]
+    double* ckey = kkey + 2 * N;                       // gathered [tile], sorted [tile]
+    double* skey = ckey + kWorldTile;
+    int* kidx = (int*)(skey + kWorldTile);             // [2][N]
+    int* cidx = kidx + 2 * N;
+    int* sidx = cidx + kWorldTile;
+    const double sx = state[3 * b], sy = state[3 * b + 1];
+    if (tid == 0) n_cand[0] = 0;
+    __syncthreads();
+    int nk = 0;                                        // pairs kept so far (uniform across the CTA)
+    for (int base = 0, tile = 0; base < count; base += kWorldTile, tile = tile == 2 ? 0 : tile + 1) {
+      const int i = base + tid;
+      if (i < count) {
+        const size_t s = (size_t)first + i;
+        const double key = obstacle_key(shape_kind[s], shape_nv[s], shape_xy + s * RDA_MAX_EDGE * 2, sx, sy);
+        if (nk < N || key < kkey[cur * N + N - 1]) {
+          const int p = atomicAdd(&n_cand[tile], 1);
+          ckey[p] = key; cidx[p] = i;
+        }
+      }
+      // the next tile's counter was last read two tiles ago, before the previous barrier, and is next
+      // incremented after the barrier below
+      if (tid == 0) n_cand[tile == 2 ? 0 : tile + 1] = 0;
+      __syncthreads();
+      const int c = n_cand[tile];
+      if (c == 0) continue;
+      if (tid < c) {                                   // rank among the candidates: sorted copy
+        const double k = ckey[tid];
+        const int ix = cidx[tid];
+        int r = 0;
+        for (int j = 0; j < c; ++j) r += obstacle_before(ckey[j], cidx[j], k, ix);
+        skey[r] = k; sidx[r] = ix;
+      }
+      __syncthreads();
+      const int nxt = cur ^ 1;
+      const double* ok = kkey + cur * N;
+      const int* oi = kidx + cur * N;
+      if (tid < c) {
+        const int p = tid + world_rank(ok, oi, nk, skey[tid], sidx[tid]);
+        if (p < N) { kkey[nxt * N + p] = skey[tid]; kidx[nxt * N + p] = sidx[tid]; }
+      }
+      for (int j = tid; j < nk; j += kWorldTile) {
+        const int p = j + world_rank(skey, sidx, c, ok[j], oi[j]);
+        if (p < N) { kkey[nxt * N + p] = ok[j]; kidx[nxt * N + p] = oi[j]; }
+      }
+      nk = nk + c < N ? nk + c : N;
+      cur = nxt;
+      __syncthreads();
+    }
+    kept_idx = kidx + cur * N;
+  }
+  if (tid == 0) obs_count[b] = count;
+  const int Tc = time_varying ? T + 1 : 1;
+  for (int q = tid; q < N * Tc; q += kWorldTile) {     // one (slot, stage) copy per thread
+    const int n = q / Tc, t = q - n * Tc;
+    float* A = obs_A + (((size_t)b * N + n) * Tc + t) * E * 2;
+    float* bb = obs_b + (((size_t)b * N + n) * Tc + t) * E;
+    if (count == 0) {
+      for (int r = 0; r < E; ++r) { A[2 * r] = 0.f; A[2 * r + 1] = 0.f; bb[r] = 0.f; }
+      if (t == 0) obs_kind[(size_t)b * N + n] = RDA_OBS_POLYGON;
+      continue;
+    }
+    const int slot = n < count ? n : count - 1;        // pad by repeating the last
+    int src = kept_idx ? kept_idx[slot] : slot;
+    if (src < 0 || src >= count) src = count - 1;      // NaN keys have no order; never read outside the world
+    const size_t s = (size_t)first + src;
+    const int kind = shape_kind[s];
+    if (t == 0) obs_kind[(size_t)b * N + n] = kind;
+    obstacle_rows(kind, shape_nv[s], shape_xy + s * RDA_MAX_EDGE * 2, shape_radius[s], shape_vel[2 * s],
+                  shape_vel[2 * s + 1], t, (double)dt, E, A, bb);
+  }
+}
+
 // arrive rule (mpc.py:170-185 without gear changes) and the controls kept as next nominal (mpc.py:186)
 __global__ void k_post_process(int B, int T, int P, int goal_index_threshold, const int* near_index, float* u_opt,
                                float* cur_vel, int* arrive) {
@@ -184,6 +296,23 @@ int rda_convert_obstacles(int B, int M, int N, int T, int E, float dt, int time_
   k_convert_obstacles<<<B, RDA_MAX_SHAPES, 0, (cudaStream_t)stream>>>(B, M, N, T, E, dt, time_varying, order, state, shape_kind,
                                                                      shape_nv, shape_xy, shape_radius, shape_vel,
                                                                      shape_count, obs_A, obs_b, obs_kind, obs_count);
+  RDA_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int rda_convert_world_obstacles(int B, int W, int N, int T, int E, float dt, int time_varying, int order,
+                                const float* state, const int32_t* world_start, const int32_t* robot_world,
+                                const int32_t* shape_kind, const int32_t* shape_nv, const float* shape_xy,
+                                const float* shape_radius, const float* shape_vel, float* obs_A, float* obs_b,
+                                int32_t* obs_kind, int32_t* obs_count, void* stream) {
+  if (B < 1 || W < 1 || N < 1 || T < 1) return RDA_E_ARG;
+  if (N > RDA_MAX_WORLD_SLOTS || E < 3 || E > RDA_MAX_EDGE) return RDA_E_UNSUPPORTED;
+  if (!world_start || !shape_kind || !shape_nv || !shape_xy || !shape_radius || !shape_vel) return RDA_E_ARG;
+  if (!obs_A || !obs_b || !obs_kind || !obs_count || (order && !state)) return RDA_E_ARG;
+  const size_t smem = order ? (size_t)(2 * N + 2 * kWorldTile) * (sizeof(double) + sizeof(int)) : 0;
+  k_convert_world_obstacles<<<B, kWorldTile, smem, (cudaStream_t)stream>>>(
+      B, W, N, T, E, dt, time_varying, order, state, world_start, robot_world, shape_kind, shape_nv, shape_xy,
+      shape_radius, shape_vel, obs_A, obs_b, obs_kind, obs_count);
   RDA_CUDA(cudaGetLastError());
   return 0;
 }

@@ -3,6 +3,9 @@
   pre_process_batch        MPC.pre_process                         (mpc.py:251-291, 338-438)
   convert_obstacles_batch  MPC.convert_rda_obstacle + RDA_solver.assign_obstacle_parameter
                            (mpc.py:189-218, 440-549; rda_solver.py:483-526)
+  convert_world_obstacles_batch
+                           the same over obstacle worlds of any size shared by many robots: each
+                           robot's N nearest shapes of its world
   BatchedMPC               MPC.control for B robots on one reference path (mpc.py:127-187),
                            closed loop without a host round trip
 
@@ -35,6 +38,31 @@ def path_tensor(ref_path, device):
     return torch.as_tensor(arr, dtype=torch.float32, device=device).contiguous()
 
 
+def _shape_arrays(*lead):
+    return {'kind': np.zeros(lead, np.int32), 'nv': np.zeros(lead, np.int32),
+            'xy': np.zeros(lead + (_cabi.MAX_EDGE, 2), np.float32), 'radius': np.zeros(lead, np.float32),
+            'vel': np.zeros(lead + (2,), np.float32)}
+
+
+def _pack_shape(out, at, o, max_edge_num):
+    """One simulator obstacle into entry `at` of the shape arrays `out`."""
+    vel = getattr(o, 'velocity', None)
+    if vel is not None:
+        out['vel'][at] = np.asarray(vel, float).reshape(-1)[:2]
+    if o.cone_type == 'norm2':
+        out['kind'][at] = _cabi.OBS_CIRCLE
+        out['xy'][at + (0,)] = np.asarray(o.center, float).reshape(-1)[:2]
+        out['radius'][at] = o.radius
+    else:
+        v = np.asarray(o.vertex, float)
+        n = v.shape[1]
+        if n > min(max_edge_num, _cabi.MAX_EDGE) or n < 3:
+            raise ValueError(f'polygon with {n} vertices: 3..{min(max_edge_num, _cabi.MAX_EDGE)} supported')
+        out['kind'][at] = _cabi.OBS_POLYGON
+        out['nv'][at] = n
+        out['xy'][at + (slice(0, n),)] = v[0:2].T
+
+
 def pack_shapes(obstacle_lists, max_shapes=None, max_edge_num=_cabi.MAX_EDGE):
     """Per-instance lists of simulator obstacles (attributes cone_type, center, radius, vertex,
     velocity — what MPC.convert_rda_obstacle reads, mpc.py:189-208) -> dict of host arrays in
@@ -44,29 +72,34 @@ def pack_shapes(obstacle_lists, max_shapes=None, max_edge_num=_cabi.MAX_EDGE):
     M = max_shapes or max(1, max(len(l) for l in obstacle_lists))
     if M > _cabi.MAX_SHAPES:
         raise ValueError(f'at most {_cabi.MAX_SHAPES} raw obstacles per instance')
-    out = {'kind': np.zeros((B, M), np.int32), 'nv': np.zeros((B, M), np.int32),
-           'xy': np.zeros((B, M, _cabi.MAX_EDGE, 2), np.float32), 'radius': np.zeros((B, M), np.float32),
-           'vel': np.zeros((B, M, 2), np.float32), 'count': np.zeros(B, np.int32)}
+    out = _shape_arrays(B, M)
+    out['count'] = np.zeros(B, np.int32)
     for b, lst in enumerate(obstacle_lists):
         if len(lst) > M:
             raise ValueError('more obstacles than max_shapes')
         out['count'][b] = len(lst)
         for j, o in enumerate(lst):
-            vel = getattr(o, 'velocity', None)
-            if vel is not None:
-                out['vel'][b, j] = np.asarray(vel, float).reshape(-1)[:2]
-            if o.cone_type == 'norm2':
-                out['kind'][b, j] = _cabi.OBS_CIRCLE
-                out['xy'][b, j, 0] = np.asarray(o.center, float).reshape(-1)[:2]
-                out['radius'][b, j] = o.radius
-            else:
-                v = np.asarray(o.vertex, float)
-                n = v.shape[1]
-                if n > min(max_edge_num, _cabi.MAX_EDGE) or n < 3:
-                    raise ValueError(f'polygon with {n} vertices: 3..{min(max_edge_num, _cabi.MAX_EDGE)} supported')
-                out['kind'][b, j] = _cabi.OBS_POLYGON
-                out['nv'][b, j] = n
-                out['xy'][b, j, :n] = v[0:2].T
+            _pack_shape(out, (b, j), o, max_edge_num)
+    return out
+
+
+def pack_worlds(worlds, max_edge_num=_cabi.MAX_EDGE):
+    """W lists of simulator obstacles (as pack_shapes takes them), each shared by any number of robots, of any
+    size -> dict of host arrays in the layout of rda_convert_world_obstacles: kind, nv, xy, radius, vel over the
+    flat list of all worlds' shapes, and start [W+1] (world w is shapes start[w]:start[w+1]).  The shape arrays
+    have at least one entry, so that a set of empty worlds still has device buffers to point at."""
+    sizes = [len(l) for l in worlds]
+    if not sizes:
+        raise ValueError('at least one world')
+    start = np.zeros(len(worlds) + 1, np.int64)
+    start[1:] = np.cumsum(sizes)
+    if start[-1] > np.iinfo(np.int32).max:
+        raise ValueError('more than 2**31 - 1 shapes')
+    out = _shape_arrays(max(1, int(start[-1])))
+    for w, lst in enumerate(worlds):
+        for j, o in enumerate(lst):
+            _pack_shape(out, (int(start[w]) + j,), o, max_edge_num)
+    out['start'] = start.astype(np.int32)
     return out
 
 
@@ -104,6 +137,29 @@ def convert_obstacles_batch(shapes, state, N, T, E, dt, time_varying=False, orde
                                               _ptr(shapes['radius']), _ptr(shapes['vel']), _ptr(shapes['count']),
                                               _ptr(A), _ptr(b), _ptr(kind), _ptr(count), _stream(dev)),
                     'rda_convert_obstacles')
+    return A, b, kind, count
+
+
+def convert_world_obstacles_batch(world, state, robot_world, N, T, E, dt, time_varying=False, order=True):
+    """world: dict of CUDA tensors from pack_worlds (kind, nv [S] int32; xy [S,8,2]; radius [S]; vel [S,2];
+    start [W+1] int32); robot_world [B] int32 or None (every robot in world 0).  Each robot gets the N nearest
+    shapes of its world (order) or its first N, as convert_obstacles_batch would given the whole world as its
+    list.  Returns obs_A [B,N,Tc,E,2], obs_b [B,N,Tc,E], obs_kind [B,N], obs_count [B] (the world sizes)."""
+    lib = _cabi.load()
+    dev = state.device
+    B, W = state.shape[0], world['start'].shape[0] - 1
+    Tc = T + 1 if time_varying else 1
+    A = torch.empty((B, N, Tc, E, 2), dtype=torch.float32, device=dev)
+    b = torch.empty((B, N, Tc, E), dtype=torch.float32, device=dev)
+    kind = torch.empty((B, N), dtype=torch.int32, device=dev)
+    count = torch.empty(B, dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        _cabi.check(lib.rda_convert_world_obstacles(B, W, N, T, E, dt, int(time_varying), int(order), _ptr(state),
+                                                    _ptr(world['start']), _ptr(robot_world), _ptr(world['kind']),
+                                                    _ptr(world['nv']), _ptr(world['xy']), _ptr(world['radius']),
+                                                    _ptr(world['vel']), _ptr(A), _ptr(b), _ptr(kind), _ptr(count),
+                                                    _stream(dev)),
+                    'rda_convert_world_obstacles')
     return A, b, kind, count
 
 
@@ -160,11 +216,20 @@ class BatchedMPC:
                            torch.zeros(B, dtype=torch.int32, device=dev))
         return self._empty
 
-    def control(self, state, ref_speed=5.0, shapes=None, time_varying=False):
+    def control(self, state, ref_speed=5.0, shapes=None, time_varying=False, world=None, robot_world=None):
         """state [B,3] (CUDA tensor or array), ref_speed scalar or [B], shapes: dict from
-        pack_shapes / shapes_to_device (None: free space).  Returns (u0 [B,2], info) where info holds
+        pack_shapes / shapes_to_device (None: free space).  Instead of shapes, world: dict from
+        pack_worlds / shapes_to_device, obstacle maps shared by the robots, with robot_world [B] the map of
+        each robot (may be omitted with a single map).  Returns (u0 [B,2], info) where info holds
         the solver's batched outputs plus 'arrive', 'nom_s', 'ref_s', 'cur_index'.  No host sync."""
         dev, B, T = self.device, self.batch, self.T
+        if world is not None:
+            if shapes is not None:
+                raise ValueError('pass either shapes or world, not both')
+            if robot_world is None and world['start'].shape[0] != 2:
+                raise ValueError('robot_world is required with more than one world')
+            if robot_world is not None:
+                robot_world = torch.as_tensor(robot_world, dtype=torch.int32, device=dev).reshape(B).contiguous()
         state = torch.as_tensor(state, dtype=torch.float32, device=dev).reshape(B, -1)[:, :3].contiguous()
         if not isinstance(ref_speed, torch.Tensor):
             ref_speed = torch.full((B,), float(ref_speed), dtype=torch.float32, device=dev) if np.isscalar(ref_speed) \
@@ -186,9 +251,12 @@ class BatchedMPC:
             nom_s, ref_s, near = pre_process_batch(state, self.cur_vel, ref_speed, self.path, self.cur_index,
                                                    self.dynamics, self.dt, self.L, T)
         self.cur_index = near
-        if shapes is None or self.N == 0:
+        if (shapes is None and world is None) or self.N == 0:
             A, b, kind, count = self._no_obstacles()
             time_varying = False
+        elif world is not None:
+            A, b, kind, count = convert_world_obstacles_batch(world, state, robot_world, self.N, T, self.E, self.dt,
+                                                              time_varying, self.obstacle_order)
         else:
             A, b, kind, count = convert_obstacles_batch(shapes, state, self.N, T, self.E, self.dt, time_varying,
                                                         self.obstacle_order)
