@@ -94,7 +94,7 @@ static int su_impl(const SuParams* P, const double* lins, const double* linu, co
   for (int i = 0; i < N * T; ++i) { W.hx[i] = hx[i]; W.hy[i] = hy[i]; W.hc[i] = hc[i]; }
   W.vref = (Real)vref;
   SeqCtx ctx;
-  int st = su_solve<Real, Real, SeqCtx>(*P, W, ctx, gx, gy, iters);
+  int st = su_solve<Real, SeqCtx>(*P, W, ctx, gx, gy, iters);
   for (int i = 0; i < 3 * (T + 1); ++i) s[i] = W.s[i];
   for (int i = 0; i < 2 * T; ++i) u[i] = W.u[i];
   for (int i = 0; i < T; ++i) d[i] = W.d[i];
@@ -195,10 +195,6 @@ int shim_su_f(const SuParams* P, const double* lins, const double* linu, const d
 static long long g_su_hist[64];
 extern "C" void port_su_hist(long long* out, int reset) { for (int i = 0; i < 64; ++i) { out[i] = g_su_hist[i]; if (reset) g_su_hist[i] = 0; } }
 
-extern "C" int shim_su_batched_fwd(const SuParams* Pin, int nb, float* cur_s, float* cur_u, const float* ref_s, const float* pref,
-                                   const float* coef, float* dis, const float* ref_speed, const int* done, int* status, int* iters,
-                                   int* counters, int max_iter);
-
 // ------------------------------------------------------------------------------------------------
 // Whole hot path on the CPU (mirrors rda_kernels.cu; see the kernel comments for reference lines).
 // Layouts as in include/rda_b200.h.  Every instance starts cold (constructor state).
@@ -235,7 +231,6 @@ extern "C" int port_solve_batch(const rda_config* cfg, const rda_tunables* tun, 
 #ifdef RDA_CELL_STATS
     std::vector<int> featv(NT > 0 ? NT : 1, 0);
 #endif
-    const bool use_batched = getenv("RDA_PORT_SU_BATCHED") && atoi(getenv("RDA_PORT_SU_BATCHED")) != 0;
     const bool use_lean2 = getenv("RDA_PORT_LEAN2") && atoi(getenv("RDA_PORT_LEAN2")) != 0;
     std::vector<int> feat2(NT > 0 ? NT : 1, 0);
     std::vector<ObstacleGeom<4>> og2(N > 0 ? N : 1);
@@ -257,18 +252,7 @@ extern "C" int port_solve_batch(const rda_config* cfg, const rda_tunables* tun, 
       W.vref = ref_speed[b];
       SeqCtx ctx;
       int nit = 0;
-      int st;
-      if (use_batched) {
-        // the batched pipeline works on the product layouts directly (and writes cs / cu / dis itself)
-        int stat = 0, itc = 0, cnt[8] = {0, 0, 0, 0, 0, 0, 0, 0}, dn = 0;
-        shim_su_batched_fwd(&P, 1, cs.data(), cu.data(), rf, pref.data(), coef.data(), dis.data(), ref_speed + b, &dn, &stat, &itc, cnt, 28);
-        nit = cnt[3];
-        st = (stat & RDA_ST_SU_NONFINITE) ? 2 : ((stat & RDA_ST_SU_NOT_CONVERGED) ? 1 : 0);
-        for (int i = 0; i < 3 * (T + 1); ++i) { int r = i / (T + 1), t = i % (T + 1); W.s[3 * t + r] = cs[i]; }
-        for (int i = 0; i < 2 * T; ++i) { int r = i / T, t = i % T; W.u[2 * t + r] = cu[i]; }
-        for (int t = 0; t < T; ++t) W.d[t] = dis[t];
-      } else
-      st = su_solve<double, double, SeqCtx>(P, W, ctx, coef.data() + 3 * NT, coef.data() + 4 * NT, &nit);
+      const int st = su_solve<double, SeqCtx>(P, W, ctx, coef.data() + 3 * NT, coef.data() + 4 * NT, &nit);
       su_iters += nit;
       if (W.restarts) {
 #pragma omp atomic
@@ -368,69 +352,6 @@ extern "C" int port_solve_batch(const rda_config* cfg, const rda_tunables* tun, 
 }
 
 
-// ---- serial launch emulation of the batched su-QP pipeline (rda_planner_b200/csrc/su_batched.cuh) --------
-// The kernels of that file have no shared memory and no intra-block synchronisation, so running their
-// bodies once per (block, thread) index reproduces the device arithmetic exactly (up to libm vs CUDA math).
-namespace emu {
-struct Dim { int x = 0, y = 0, z = 0; };
-static thread_local Dim blockIdx, threadIdx, blockDim;
-static inline int atomicAdd(int* p, int v) { int o = *p; *p += v; return o; }
-static inline int atomicSub(int* p, int v) { int o = *p; *p -= v; return o; }
-}
-#define RDA_SB_EMULATE 1
-#define __global__
-#define __device__
-#define __forceinline__ inline
-#define __launch_bounds__(...)
-using emu::blockIdx; using emu::threadIdx; using emu::blockDim; using emu::atomicAdd; using emu::atomicSub;
-#include "../../rda_planner_b200/csrc/su_batched.cuh"
-#undef __global__
-#undef __device__
-#undef __forceinline__
-#undef __launch_bounds__
-
-template <typename F> static void emu_launch(int gx, int gy, int bx, F&& body) {
-  emu::blockDim.x = bx;
-  for (int y = 0; y < gy; ++y)
-    for (int x = 0; x < gx; ++x)
-      for (int t = 0; t < bx; ++t) { emu::blockIdx.x = x; emu::blockIdx.y = y; emu::threadIdx.x = t; body(); }
-}
-
-// nb instances, product layouts (include/rda_b200.h): cur_s/ref_s [nb][3][T+1], cur_u/pref [nb][2][T],
-// coef [nb][5][N][T], dis [nb][T].  Outputs in place (cur_s, cur_u, dis) + status / iters / counters[8].
-extern "C" int shim_su_batched(const SuParams* Pin, int nb, float* cur_s, float* cur_u, const float* ref_s,
-                               const float* pref, const float* coef, float* dis, const float* ref_speed,
-                               const int* done, int* status, int* iters, int* counters, int max_iter) {
-  SuParams P = *Pin;
-  P.max_iter = max_iter;
-  const int T = P.T, N = P.N;
-  const size_t bytes = su_batch_layout(nb, T, N, nullptr, nullptr);
-  std::vector<char> buf(bytes + 512, 0);
-  char* base = (char*)(((uintptr_t)buf.data() + 255) & ~(uintptr_t)255);
-  SuBatch W;
-  su_batch_layout(nb, T, N, &W, base);
-  *W.n_active = 0;
-  const double Mrows = 4.0 * T + (N > 0 ? 2.0 * T : 0.0) + 4.0 * (T - 1) + (P.accelerated ? (double)N * T : 0.0);
-  SbOut out{cur_s, cur_u, dis, status, iters, counters};
-  const int gs = (nb + 127) / 128, gi = (nb + 31) / 32;
-  emu_launch(gs, T, 128, [&] { ksb_setup(W, P, cur_s, cur_u, ref_s, pref, coef, dis, ref_speed, done); });
-  emu_launch(1, 1, 1, [&] { ksb_compact(W); });
-  emu_launch(gi, 1, 32, [&] { ksb_rollout(W); });
-  for (int it = 0; it <= P.max_iter; ++it) {
-    emu_launch(gs, T, 128, [&] { ksb_assemble(W, P, it); });
-    emu_launch(gi, 1, 32, [&] { ksb_riccati<true>(W, P, it, Mrows, out); });
-    emu_launch(1, 1, 1, [&] { ksb_compact(W); });
-    if (it == P.max_iter) break;
-    emu_launch(gs, T, 128, [&] { ksb_steplen<0>(W, P, it); });
-    emu_launch(gs, 1, 128, [&] { ksb_reduce<0>(W, Mrows); });
-    emu_launch(gs, T, 128, [&] { ksb_corrector(W, P, it); });
-    emu_launch(gi, 1, 32, [&] { ksb_riccati<false>(W, P, it, Mrows, out); });
-    emu_launch(gs, T, 128, [&] { ksb_steplen<1>(W, P, it); });
-    emu_launch(gs, 1, 128, [&] { ksb_reduce<1>(W, Mrows); });
-  }
-  return *W.n_active;
-}
-
 // ---- front end cores (rda_planner_b200/csrc/frontend.cuh), one instance per call -----------------
 #include "../../rda_planner_b200/csrc/frontend.cuh"
 
@@ -503,9 +424,3 @@ extern "C" void port_coh_stats(long long* out) { memcpy(out, g_coh, sizeof(g_coh
 extern "C" void port_cell_stats(long long* out) { memcpy(out, g_stat_hist, sizeof(g_stat_hist)); }
 extern "C" void port_cell_situations(long long* out) { memcpy(out, rda::g_cell_stats, sizeof(rda::g_cell_stats)); }
 #endif
-
-extern "C" int shim_su_batched_fwd(const SuParams* Pin, int nb, float* cur_s, float* cur_u, const float* ref_s, const float* pref,
-                                   const float* coef, float* dis, const float* ref_speed, const int* done, int* status, int* iters,
-                                   int* counters, int max_iter) {
-  return shim_su_batched(Pin, nb, cur_s, cur_u, ref_s, pref, coef, dis, ref_speed, done, status, iters, counters, max_iter);
-}

@@ -14,18 +14,11 @@
 #include "rda_hd.h"
 #include "cell_solver.cuh"
 #include "su_solver.cuh"
-#include "su_batched.cuh"
 #include "cell_lean.cuh"
 #include "cell_lean2.cuh"
 #include "cell_disc_robot.cuh"
 
 using namespace rda;
-
-// Lanes per planning instance in the su-QP kernel: 32 = one warp per instance (lowest latency, everything in
-// shared memory); 16 / 8 = 2 / 4 instances share a warp.  The serial Riccati recursion is executed by every
-// lane of a group, so a narrower group wastes fewer issue slots on it; the kernel is latency bound at the
-// ~12 warps per SM that registers allow, so more instances per warp is more throughput once the batch is
-// large enough to fill the SMs (su_group_for).
 
 // byte offsets of the persistent kernel's shared-memory state (k_admm_small)
 struct SmallLayout {
@@ -42,13 +35,8 @@ struct rda_handle {
   float *resi_acc, *resi_pri, *resi_dual;
   int *status, *iters, *done, *counters, *worklist, *worklist2;
   char* su_ws;           // [B][su_ws_stride] global workspace of the su-QP interior point iteration (hinge slacks /
-                         // multipliers; for sub-warp groups also the Riccati gains and the stage arrays)
+                         // multipliers)
   size_t su_ws_stride;
-  char* sb_ws;           // workspace of the batched su-QP pipeline (su_batched.cuh), allocated on first use
-  size_t sb_bytes, sb_slab;
-  int su_batched;        // -1: by sub-batch size (>= su_batched_min instances), 0: never, 1: always (RDA_B200_SU_BATCHED)
-  int su_batched_min;
-  int su_group;          // lanes per instance in k_su: 0 = by sub-batch size, else 32 / 16 / 8 (RDA_B200_SU_GROUP)
   // coherent first cell pass (cell_lean2.cuh; RDA_B200_LEAN2=1, E <= 4, R <= 4, static obstacles)
   int lean2;
   RobotAux ra;
@@ -72,7 +60,6 @@ struct rda_handle {
   int small_max, small_ok, small_bulk;
   int small_coop;        // interior point cells of the persistent kernel one per warp (RDA_B200_SMALL_COOP, default 1)
   SmallLayout small_L;
-  int su_maxctas;        // cap on resident k_su CTAs per SM in split mode (0 = none; RDA_B200_SU_MAXCTAS)
   float su_prune;        // hinge pruning margin of the su-QP (su_solver.cuh; RDA_B200_SU_PRUNE, 0 = off)
   int slow_cpw, slow_ctas;   // k_cells_slow: cells per warp, CTAs per SM (RDA_B200_SLOW_CPW / RDA_B200_SLOW_CTAS)
   int slow_coop;             // warp-cooperative last pass, one cell per warp (RDA_B200_SLOW_COOP, default 1)
@@ -88,30 +75,21 @@ struct rda_handle {
 
 namespace {
 
-// Sub-warp group of G lanes (G = 16, 8): several instances share one warp.  All synchronisation and
-// shuffles use the group's own lane mask, so the groups of a warp may diverge (different interior
-// point iteration counts) and re-converge freely (independent thread scheduling); while they run in
-// lock-step one FP64 instruction serves G-lane pieces of several instances.
-template <int G>
-struct GroupCtx {
-  unsigned mask;
-  __device__ __forceinline__ GroupCtx() {
-    const int l = threadIdx.x & 31;
-    mask = (G == 32) ? 0xffffffffu : (((1u << G) - 1u) << (l / G * G));
-  }
-  __device__ __forceinline__ int lane() const { return threadIdx.x & (G - 1); }
-  __device__ __forceinline__ int nlanes() const { return G; }
-  __device__ __forceinline__ void sync() const { __syncwarp(mask); }
+// The cooperative context of one whole warp (su_solver.cuh, coop_ipm.cuh): lanes, warp barrier, butterfly reductions.
+struct WarpCtx {
+  __device__ __forceinline__ int lane() const { return threadIdx.x & 31; }
+  __device__ __forceinline__ int nlanes() const { return 32; }
+  __device__ __forceinline__ void sync() const { __syncwarp(); }
   template <typename R> __device__ __forceinline__ R sum(R x) const {
-    for (int o = G / 2; o > 0; o >>= 1) x += __shfl_xor_sync(mask, x, o);
+    for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
     return x;
   }
   template <typename R> __device__ __forceinline__ R min(R x) const {
-    for (int o = G / 2; o > 0; o >>= 1) { R y = __shfl_xor_sync(mask, x, o); x = y < x ? y : x; }
+    for (int o = 16; o > 0; o >>= 1) { R y = __shfl_xor_sync(0xffffffffu, x, o); x = y < x ? y : x; }
     return x;
   }
   template <typename R> __device__ __forceinline__ R max(R x) const {
-    for (int o = G / 2; o > 0; o >>= 1) { R y = __shfl_xor_sync(mask, x, o); x = y > x ? y : x; }
+    for (int o = 16; o > 0; o >>= 1) { R y = __shfl_xor_sync(0xffffffffu, x, o); x = y > x ? y : x; }
     return x;
   }
 };
@@ -153,41 +131,41 @@ __global__ void k_begin(DevPtrs d, const float* nom_s, const float* nom_u, const
 
 // The su-QP of instance b: inputs from the persistent state (d), solve (su_solver.cuh), accepted result back.
 // W is laid out by the caller (hs / hnu and the workspace may live in shared or global memory).
-template <typename Real, int G>
-__device__ __forceinline__ void su_instance(const DevPtrs& d, const SuParams& P, int b, SuWork<Real, Real>& W, GroupCtx<G>& ctx) {
+template <typename Real>
+__device__ __forceinline__ void su_instance(const DevPtrs& d, const SuParams& P, int b, SuWork<Real>& W, WarpCtx& ctx) {
   const int T = P.T, N = P.N, NT = N * T;
   const int lane = ctx.lane();
   const float* cs = d.cur_s + (size_t)b * 3 * (T + 1);   // [3][T+1]
   const float* cu = d.cur_u + (size_t)b * 2 * T;         // [2][T]
   const float* rf = d.ref_s + (size_t)b * 3 * (T + 1);
-  for (int i = lane; i < 3 * (T + 1); i += G) {
+  for (int i = lane; i < 3 * (T + 1); i += 32) {
     int r = i / (T + 1), t = i - r * (T + 1);
     W.lins[3 * t + r] = cs[i];
     W.ref[3 * t + r] = rf[i];
   }
-  for (int i = lane; i < 2 * T; i += G) {
+  for (int i = lane; i < 2 * T; i += 32) {
     int r = i / T, t = i - r * T;
     W.linu[2 * t + r] = cu[i];
     W.pref[2 * t + r] = d.pref[(size_t)b * 2 * T + i];
   }
-  for (int t = lane; t < T; t += G) W.d[t] = d.dis[(size_t)b * T + t];
+  for (int t = lane; t < T; t += 32) W.d[t] = d.dis[(size_t)b * T + t];
   float* cf = d.coef + (size_t)b * 5 * NT;
   W.hx = cf; W.hy = cf + NT; W.hc = cf + 2 * NT;
   W.vref = d.ref_speed[b];
   ctx.sync();
   int iters = 0;
-  int st = su_solve<Real, Real, GroupCtx<G>>(P, W, ctx, cf + 3 * NT, cf + 4 * NT, &iters);
+  int st = su_solve<Real, WarpCtx>(P, W, ctx, cf + 3 * NT, cf + 4 * NT, &iters);
   ctx.sync();
   // accept OPTIMAL and OPTIMAL_INACCURATE (iteration cap), else keep the previous nominal
   // ("No update of state and control vector", rda_solver.py:696-700)
   bool ok = st != 2;
   if (ok) {
-    for (int i = lane; i < 3 * (T + 1); i += G) {
+    for (int i = lane; i < 3 * (T + 1); i += 32) {
       int r = i / (T + 1), t = i - r * (T + 1);
       float v = (float)W.s[3 * t + r];
       if (!isfinite(v)) ok = false;
     }
-    for (int i = lane; i < 2 * T; i += G) {
+    for (int i = lane; i < 2 * T; i += 32) {
       int r = i / T, t = i - r * T;
       if (!isfinite((float)W.u[2 * t + r])) ok = false;
     }
@@ -196,15 +174,15 @@ __device__ __forceinline__ void su_instance(const DevPtrs& d, const SuParams& P,
   if (ok) {
     float* ws = d.cur_s + (size_t)b * 3 * (T + 1);
     float* wu = d.cur_u + (size_t)b * 2 * T;
-    for (int i = lane; i < 3 * (T + 1); i += G) {
+    for (int i = lane; i < 3 * (T + 1); i += 32) {
       int r = i / (T + 1), t = i - r * (T + 1);
       ws[i] = (float)W.s[3 * t + r];
     }
-    for (int i = lane; i < 2 * T; i += G) {
+    for (int i = lane; i < 2 * T; i += 32) {
       int r = i / T, t = i - r * T;
       wu[i] = (float)W.u[2 * t + r];
     }
-    for (int t = lane; t < T; t += G) d.dis[(size_t)b * T + t] = (float)W.d[t];
+    for (int t = lane; t < T; t += 32) d.dis[(size_t)b * T + t] = (float)W.d[t];
   }
   if (lane == 0) {
     d.iters[b] += 1;
@@ -221,35 +199,18 @@ __device__ __forceinline__ void su_instance(const DevPtrs& d, const SuParams& P,
 // ------------------------------------------------------------------------------------------------
 // K1: su-QP, one warp per instance.
 // ------------------------------------------------------------------------------------------------
-// Build-time experiment knobs (third session of round 2): RDA_SU_BSG = 1 keeps the box slacks / multipliers of the one-warp
-// variant in global memory ([c][t], coalesced) — 13.2 instead of 17.9 KB of shared memory per instance at the metric size;
-// RDA_SU_MINCTAS = n asks the compiler for n resident CTAs per SM (16 needs <= 128 registers).  Both off by default.
-#ifdef RDA_SU_MINCTAS
-#define RDA_SU_BOUNDS __launch_bounds__(32, RDA_SU_MINCTAS)
-#else
-#define RDA_SU_BOUNDS __launch_bounds__(32)
-#endif
-template <typename Real, int G>
-__global__ void RDA_SU_BOUNDS k_su(DevPtrs d, SuParams P, int smem_per_instance) {
-  constexpr int LEVEL = G == 32 ? 0 : (G == 16 ? 1 : 2);      // workspace placement of sub-warp groups (su_work_layout)
-  constexpr bool BSG = G == 32 && RDA_SU_BSG != 0;
+template <typename Real>
+__global__ void __launch_bounds__(32) k_su(DevPtrs d, SuParams P) {
   extern __shared__ __align__(16) char smem[];
-  constexpr int PER_WARP = 32 / G;
-  const int grp = (threadIdx.x & 31) / G;
-  const int b = blockIdx.x * PER_WARP + grp;
+  const int b = blockIdx.x;
   if (b >= d.B) return;
   if (d.done[b]) return;
-  GroupCtx<G> ctx;
-  const int T = P.T, N = P.N, NT = N * T;
-  const int lane = ctx.lane();
-  SuWork<Real, Real> W;
+  WarpCtx ctx;
+  SuWork<Real> W;
   // per-hinge data stays in global memory (L2): every entry is touched only by the lane that owns
-  // its stage, consecutive lanes read consecutive addresses.  With sub-warp groups (level > 0) the
-  // Riccati gains / stage arrays live there too, so that shared memory does not limit the number of
-  // resident instances.
-  su_work_layout<Real, Real, LEVEL, BSG>(T, N, &W, smem + (size_t)grp * smem_per_instance, false,
-                                         d.su_ws + (size_t)b * d.su_ws_stride);
-  su_instance<Real, G>(d, P, b, W, ctx);
+  // its stage, consecutive lanes read consecutive addresses
+  su_work_layout<Real>(P.T, P.N, &W, smem, false, d.su_ws + (size_t)b * d.su_ws_stride);
+  su_instance<Real>(d, P, b, W, ctx);
 }
 
 // inputs of one cell gathered from the persistent state
@@ -796,7 +757,7 @@ __global__ void __launch_bounds__(32 * DR_COOP_WARPS) k_cells_dr_slow_coop(DevPt
   const int count = d.wl_count[4];          // what k_cells_dr_mid left, in d.worklist
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   DiscSlowStore& S = store[warp];
-  GroupCtx<32> ctx;
+  WarpCtx ctx;
   for (int wi = blockIdx.x * DR_COOP_WARPS + warp; wi < count; wi += gridDim.x * DR_COOP_WARPS) {
     const long long idx = d.worklist[wi];
     CellIn c;
@@ -810,7 +771,7 @@ __global__ void __launch_bounds__(32 * DR_COOP_WARPS) k_cells_dr_slow_coop(DevPt
     const int have = __shfl_sync(0xffffffffu, (int)w.have, 0);
     if (!have) {
       __syncwarp();
-      cell_slow_dr<float, GroupCtx<32>>(rb, w, S, ctx);
+      cell_slow_dr<float, WarpCtx>(rb, w, S, ctx);
       __syncwarp();
     }
     if (lane == 0) {
@@ -886,7 +847,7 @@ __global__ void __launch_bounds__(32 * SLOW_COOP_WARPS) k_cells_slow_coop(DevPtr
   const int* list = from_extra ? d.worklist : d.worklist2;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   CellSlowStore& S = store[warp];
-  GroupCtx<32> ctx;
+  WarpCtx ctx;
   for (int wi = blockIdx.x * SLOW_COOP_WARPS + warp; wi < count; wi += gridDim.x * SLOW_COOP_WARPS) {
     const long long idx = list[wi];
     CellIn c;
@@ -899,7 +860,7 @@ __global__ void __launch_bounds__(32 * SLOW_COOP_WARPS) k_cells_slow_coop(DevPtr
     const int have = __shfl_sync(0xffffffffu, (int)w.have, 0);
     if (!have) {
       __syncwarp();
-      cell_slow<float, GroupCtx<32>>(rb, w, S, ctx);
+      cell_slow<float, WarpCtx>(rb, w, S, ctx);
       __syncwarp();
     }
     if (lane == 0) {
@@ -1065,10 +1026,10 @@ __global__ void __launch_bounds__(128) k_admm_small(DevPtrs d, SuParams P, Robot
   const bool has_obs = N > 0 && ds.obs_count[0] != 0;
   for (int it = 0; it < iter_num; ++it) {
     if (tid < 32) {
-      GroupCtx<32> ctx;
-      SuWork<Real, Real> W;
-      su_work_layout<Real, Real, 0>(T, N, &W, smem + L.su, false, smem + L.hs);
-      su_instance<Real, 32>(ds, P, 0, W, ctx);
+      WarpCtx ctx;
+      SuWork<Real> W;
+      su_work_layout<Real>(T, N, &W, smem + L.su, false, smem + L.hs);
+      su_instance<Real>(ds, P, 0, W, ctx);
     }
     __syncthreads();
     if (has_obs) {
@@ -1104,7 +1065,7 @@ __global__ void __launch_bounds__(128) k_admm_small(DevPtrs d, SuParams P, Robot
         __syncthreads();
         const int nlist = wl[0], warp = tid >> 5, lane = tid & 31;
         CellSlowStore& S = ((CellSlowStore*)(smem + L.slow))[warp];
-        GroupCtx<32> ctx;
+        WarpCtx ctx;
         for (int wi = warp; wi < nlist; wi += (nth >> 5)) {
           const int idx = wl[1 + wi];
           CellIn c;
@@ -1115,7 +1076,7 @@ __global__ void __launch_bounds__(128) k_admm_small(DevPtrs d, SuParams P, Robot
             cell_front<float, false, true>(rb, c.kind, E, c.A, c.bb, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0, c.xi1, ro2, w);
           }
           __syncwarp();
-          cell_slow<float, GroupCtx<32>>(rb, w, S, ctx);
+          cell_slow<float, WarpCtx>(rb, w, S, ctx);
           __syncwarp();
           if (lane == 0) {
             CellOut<float> o;
@@ -1281,19 +1242,11 @@ int rda_create(const rda_config* cfg, const rda_tunables* tun, rda_handle** out)
   h->R = cfg->robot_edges;
   const size_t B = h->B, T = h->T, N = h->N, E = h->E, R = h->R, NT = N * T;
   {
-    // largest global slab any placement level needs (sub-warp groups keep more of the workspace there)
-    size_t gmax = 0, g = 0, sm0;
-    if (cfg->su_fp64) {
-      sm0 = su_work_bytes<double, double, 0>((int)T, (int)N, false, &g); gmax = g;
-      su_work_bytes<double, double, 1>((int)T, (int)N, false, &g); if (g > gmax) gmax = g;
-      su_work_bytes<double, double, 2>((int)T, (int)N, false, &g); if (g > gmax) gmax = g;
-    } else {
-      sm0 = su_work_bytes<float, float, 0>((int)T, (int)N, false, &g); gmax = g;
-      su_work_bytes<float, float, 1>((int)T, (int)N, false, &g); if (g > gmax) gmax = g;
-      su_work_bytes<float, float, 2>((int)T, (int)N, false, &g); if (g > gmax) gmax = g;
-    }
-    if (sm0 > 227 * 1024) { delete h; return RDA_E_UNSUPPORTED; }
-    h->su_ws_stride = (gmax + 127) & ~(size_t)127;
+    // k_su keeps its workspace in shared memory, the hinge slacks / multipliers in a global slab per instance
+    size_t g = 0;
+    const size_t sm = cfg->su_fp64 ? su_work_bytes<double>((int)T, (int)N, false, &g) : su_work_bytes<float>((int)T, (int)N, false, &g);
+    if (sm > 227 * 1024) { delete h; return RDA_E_UNSUPPORTED; }
+    h->su_ws_stride = (g + 127) & ~(size_t)127;
   }
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
@@ -1311,33 +1264,8 @@ int rda_create(const rda_config* cfg, const rda_tunables* tun, rda_handle** out)
   alloc((float**)&h->worklist2, B * NT);
   alloc((float**)&h->su_ws, B * (h->su_ws_stride / 4));
   if (e != cudaSuccess) { rda_destroy(h); return (int)e; }
-  {
-    const int cap = 227 * 1024;
-    if (cfg->su_fp64) {
-      e = cudaFuncSetAttribute(k_su<double, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
-      if (e == cudaSuccess) e = cudaFuncSetAttribute(k_su<double, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
-      if (e == cudaSuccess) e = cudaFuncSetAttribute(k_su<double, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
-    } else {
-      e = cudaFuncSetAttribute(k_su<float, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
-      if (e == cudaSuccess) e = cudaFuncSetAttribute(k_su<float, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
-      if (e == cudaSuccess) e = cudaFuncSetAttribute(k_su<float, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
-    }
-  }
-  h->su_group = 0;
-  if (const char* g = getenv("RDA_B200_SU_GROUP")) { int v = atoi(g); if (v == 32 || v == 16 || v == 8) h->su_group = v; }
-  h->su_batched = 0; h->su_batched_min = 3072;      // measured slower than k_su (r02, DESIGN.md §4): opt-in
-  if (const char* g = getenv("RDA_B200_SU_BATCHED")) { int v = atoi(g); if (v >= -1 && v <= 1) h->su_batched = v; }
-  if (const char* g = getenv("RDA_B200_SU_BATCHED_MIN")) { int v = atoi(g); if (v >= 1) h->su_batched_min = v; }
-  if (cfg->su_fp64 && h->su_group == 0 && (h->su_batched == 1 || (h->su_batched < 0 && h->B >= h->su_batched_min))) {
-    int parts = 2;
-    if (const char* sp = getenv("RDA_B200_SPLIT_PARTS")) { int v = atoi(sp); if (v >= 1 && v <= 4) parts = v; }
-    const int nbmax = (h->B + parts - 1) / parts + 1;
-    h->sb_slab = (su_batch_layout(nbmax, (int)T, (int)N, nullptr, nullptr) + 4095) & ~(size_t)4095;
-    const size_t whole = su_batch_layout(h->B, (int)T, (int)N, nullptr, nullptr);
-    h->sb_bytes = (h->sb_slab * parts > whole ? h->sb_slab * parts : whole) + 4096;
-    e = cudaMalloc((void**)&h->sb_ws, h->sb_bytes);
-    if (e != cudaSuccess) { rda_destroy(h); return (int)e; }
-  }
+  e = cfg->su_fp64 ? cudaFuncSetAttribute(k_su<double>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)
+                   : cudaFuncSetAttribute(k_su<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
   if (e != cudaSuccess) { rda_destroy(h); return (int)e; }
   e = cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming);
   for (int p = 0; p < 3; ++p) {
@@ -1359,11 +1287,9 @@ int rda_create(const rda_config* cfg, const rda_tunables* tun, rda_handle** out)
   }
   h->split_min = 2048;
   h->parts = 2;
-  h->su_maxctas = 0;
-  if (const char* v = getenv("RDA_B200_SU_MAXCTAS")) { int x = atoi(v); if (x >= 1 && x <= 32) h->su_maxctas = x; }
   h->su_prune = 0.5f;       // chosen by a sweep of 0.5, 1, 2 and off at B = 16384
   {
-    const size_t sub = cfg->su_fp64 ? su_work_bytes<double, double, 0>((int)T, (int)N, false) : su_work_bytes<float, float, 0>((int)T, (int)N, false);
+    const size_t sub = cfg->su_fp64 ? su_work_bytes<double>((int)T, (int)N, false) : su_work_bytes<float>((int)T, (int)N, false);
     h->small_L = small_layout((int)T, (int)N, (int)E, (int)R, sub);
     h->small_ok = h->small_L.total <= 200 * 1024 && !h->rb.disc;      // the persistent kernel has the polygon body's cells only
     h->small_mode = -1; h->small_max = 2 * h->sms;      // two resident CTAs per SM
@@ -1412,7 +1338,6 @@ int rda_destroy(rda_handle* h) {
                    h->ref_s, h->ref_speed, h->resi_acc, h->resi_pri, h->resi_dual, (float*)h->status,
                    (float*)h->iters, (float*)h->done, (float*)h->counters, (float*)h->worklist, (float*)h->worklist2, (float*)h->su_ws};
   for (float* p : bufs) if (p) cudaFree(p);
-  if (h->sb_ws) cudaFree(h->sb_ws);
   if (h->ogeo) cudaFree(h->ogeo);
   if (h->feat) cudaFree(h->feat);
   if (h->worklist0) cudaFree(h->worklist0);
@@ -1492,75 +1417,14 @@ static int begin_part(rda_handle* h, const rda_inputs* in, int b0, int nb, int p
   return 0;
 }
 
-// The su-QP of a sub-batch as a pipeline of wide kernels (su_batched.cuh): chosen for large sub-batches in
-// float64, where one warp per instance leaves most of the machine idle.
-static int step_su_batched(rda_handle* h, int b0, int nb, int part, cudaStream_t s) {
-  DevPtrs d = dev_ptrs(h, b0, nb, part);
-  SuParams P = su_params(h);
-  P.max_iter = 28;
-  const int T = h->T, N = h->N;
-  // one slab per sub-batch (sb_slab bytes each); a whole-batch call (phase API) uses the workspace from 0
-  SuBatch W;
-  const size_t off = (size_t)part * h->sb_slab;
-  if (off + su_batch_layout(nb, T, N, nullptr, nullptr) > h->sb_bytes) return RDA_E_NOMEM;
-  su_batch_layout(nb, T, N, &W, h->sb_ws + off);
-  const bool acc = h->cfg.accelerated != 0;
-  const double Mrows = 4.0 * T + (N > 0 ? 2.0 * T : 0.0) + 4.0 * (T - 1) + (acc ? (double)N * T : 0.0);
-  SbOut out{d.cur_s, d.cur_u, d.dis, d.status, d.iters, d.counters};
-  const dim3 gs((nb + 127) / 128, T);
-  const int gi = (nb + 31) / 32, gr = (nb + 127) / 128;
-  ksb_setup<<<gs, 128, 0, s>>>(W, P, d.cur_s, d.cur_u, d.ref_s, d.pref, d.coef, d.dis, d.ref_speed, d.done);
-  ksb_compact<<<1, 1024, 0, s>>>(W);
-  ksb_rollout<<<gi, 32, 0, s>>>(W);
-  h->launches += 3;
-  for (int it = 0; it <= P.max_iter; ++it) {
-    ksb_assemble<<<gs, 128, 0, s>>>(W, P, it);
-    ksb_riccati<true><<<gi, 32, 0, s>>>(W, P, it, Mrows, out);
-    ksb_compact<<<1, 1024, 0, s>>>(W);
-    h->launches += 3;
-    if (it == P.max_iter) break;
-    ksb_steplen<0><<<gs, 128, 0, s>>>(W, P, it);
-    ksb_reduce<0><<<gr, 128, 0, s>>>(W, Mrows);
-    ksb_corrector<<<gs, 128, 0, s>>>(W, P, it);
-    ksb_riccati<false><<<gi, 32, 0, s>>>(W, P, it, Mrows, out);
-    ksb_steplen<1><<<gs, 128, 0, s>>>(W, P, it);
-    ksb_reduce<1><<<gr, 128, 0, s>>>(W, Mrows);
-    h->launches += 6;
-  }
-  RDA_CUDA(cudaGetLastError());
-  return 0;
-}
-
+// The su-QP of a sub-batch: one warp (one CTA) per instance.
 static int step_su_part(rda_handle* h, int b0, int nb, int part, cudaStream_t s) {
-  if (h->sb_ws && (h->su_batched == 1 || (h->su_batched < 0 && nb >= h->su_batched_min)))
-    return step_su_batched(h, b0, nb, part, s);
   DevPtrs d = dev_ptrs(h, b0, nb, part);
   SuParams P = su_params(h);
-  // group width: one warp per instance.  Narrower groups (RDA_B200_SU_GROUP=16/8: 2 / 4 instances per warp,
-  // workspace partly in global memory) were measured SLOWER, the narrower the slower: the serial Riccati
-  // recursion then waits on L2 instead of shared memory every stage.
-  int G = h->su_group;
-  if (G == 0) G = 32;
-  const int per_warp = 32 / G;
-  size_t smem1;
-  if (h->cfg.su_fp64) smem1 = G == 32 ? su_work_bytes<double, double, 0, RDA_SU_BSG != 0>(h->T, h->N, false) : (G == 16 ? su_work_bytes<double, double, 1>(h->T, h->N, false) : su_work_bytes<double, double, 2>(h->T, h->N, false));
-  else smem1 = G == 32 ? su_work_bytes<float, float, 0, RDA_SU_BSG != 0>(h->T, h->N, false) : (G == 16 ? su_work_bytes<float, float, 1>(h->T, h->N, false) : su_work_bytes<float, float, 2>(h->T, h->N, false));
-  if (smem1 * per_warp > 227 * 1024) return RDA_E_UNSUPPORTED;
-  const int grid = (nb + per_warp - 1) / per_warp;
-  size_t cta_smem = smem1 * per_warp;
-  // optional cap on the resident su-QP CTAs per SM (RDA_B200_SU_MAXCTAS): padding the dynamic shared memory leaves
-  // registers / warp slots for the latency-bound cell passes of the OTHER sub-batch to run beside this kernel
-  if (h->su_maxctas > 0 && h->B >= h->split_min && h->parts >= 2) {
-    const size_t pad = (size_t)(227 * 1024) / (size_t)h->su_maxctas - 1024;
-    if (pad > cta_smem) cta_smem = pad & ~(size_t)15;
-  }
-#define RDA_LAUNCH_SU(REAL, GG) k_su<REAL, GG><<<grid, 32, cta_smem, s>>>(d, P, (int)smem1)
-  if (h->cfg.su_fp64) {
-    if (G == 32) RDA_LAUNCH_SU(double, 32); else if (G == 16) RDA_LAUNCH_SU(double, 16); else RDA_LAUNCH_SU(double, 8);
-  } else {
-    if (G == 32) RDA_LAUNCH_SU(float, 32); else if (G == 16) RDA_LAUNCH_SU(float, 16); else RDA_LAUNCH_SU(float, 8);
-  }
-#undef RDA_LAUNCH_SU
+  const size_t smem1 = h->cfg.su_fp64 ? su_work_bytes<double>(h->T, h->N, false) : su_work_bytes<float>(h->T, h->N, false);
+  if (smem1 > 227 * 1024) return RDA_E_UNSUPPORTED;
+  if (h->cfg.su_fp64) k_su<double><<<nb, 32, smem1, s>>>(d, P);
+  else k_su<float><<<nb, 32, smem1, s>>>(d, P);
   RDA_CUDA(cudaGetLastError());
   h->launches += 1;
   return 0;

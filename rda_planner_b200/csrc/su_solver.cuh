@@ -22,25 +22,6 @@
 
 namespace rda {
 
-// Fraction to the boundary of the corrector step: 0 (default) = the fixed 0.995, which caps the decrease of the complementarity
-// at a factor 200 per iteration in the end game; K > 0 = max(0.995, 1 - K * mu).  Measured on the CPU build (third session of
-// round 2, 128 bench + 128 harsh-band instances x 50 ADMM iterations): K = 10 saves 4.4 % of the interior point iterations
-// (11.13 -> 10.64, 13.17 -> 12.67 per solve) with unchanged gaps to the float64 oracle, but CYCLES on a box-only problem
-// (no hinges, tests/test_su_batched.py [acker-0-1]: mu 2.6e-6 -> 2.4e-7 -> 1.6e-6 -> 1.5e-6 -> ... to the iteration cap) —
-// Mehrotra's single step length is fragile once iterates are pressed against the bounds.  Not adopted.
-#ifndef RDA_SU_TAU_ADAPT
-#define RDA_SU_TAU_ADAPT 0
-#endif
-// RDA_SU_BSG = 1 (build-time experiment, third session of round 2): the one-warp kernel keeps the box slacks / multipliers in
-// global memory, stored [c][t] so that the lanes (= stages) read consecutive addresses; default: [t][c] in shared memory.
-#ifndef RDA_SU_BSG
-#define RDA_SU_BSG 0
-#endif
-#if RDA_SU_BSG
-#define RDA_SU_BSI(T, t, c) ((c) * (T) + (t))
-#else
-#define RDA_SU_BSI(T, t, c) (10 * (t) + (c))
-#endif
 #ifndef RDA_SU_CH
 #define RDA_SU_CH 2      // hinges per chunk of the su-QP hinge loops (loads grouped ahead of the arithmetic)
 #endif
@@ -56,10 +37,8 @@ struct SuParams {
 };
 
 // Per-instance workspace.  All arrays indexed by stage t (0..T-1) unless noted; hinge arrays indexed
-// [o*T + t].  Real: arithmetic / iterate type; Slk: storage type of the interior point slacks and
-// multipliers (float on the GPU: they are only ever used through ratios and products, the residuals are
-// recomputed from the double iterate every iteration).
-template <typename Real, typename Slk = Real>
+// [o*T + t].  Real: arithmetic, iterate and slack / multiplier type.
+template <typename Real>
 struct SuWork {
   Real *s, *u, *d;            // iterate: 3(T+1), 2T, T
   float *ref;                 // 3(T+1)   (inputs stay in the float32 they arrive in)
@@ -68,9 +47,9 @@ struct SuWork {
   Real *Skk, *Sgk;            // aggregated rotation-consensus terms
   float *pref;                // 2T positions the hinge offsets refer to
   float *hx, *hy, *hc;        // hinge rows: lam'A (2) and offset
-  Slk *hs, *hnu;              // hinge slack / multiplier
+  Real *hs, *hnu;             // hinge slack / multiplier
   unsigned *hmask;            // T x ceil(N/32) words: hinges of stage t that take part in the interior point iteration
-  Slk *bs, *bnu;              // 10T box/rate slack / multiplier, entry (t, c) at RDA_SU_BSI(T, t, c)
+  Real *bs, *bnu;             // 10T box/rate slack / multiplier, entry (t, c) at 10 * t + c
   Real *Wm;                   // 3T hinge Hessian of the position block after the elimination of d_t (xx, xy, yy)
   Real *Ed;                   // 3T elimination of d_t: (M_xd / Q_dd, M_yd / Q_dd, 1 / Q_dd)
   Real *g5q;                  // T   reduced-out gradient of d_t: g_d / Q_dd (d step = -(g5q + Ed . dp))
@@ -89,16 +68,12 @@ struct SuWork {
 };
 
 // Workspace placement.  `base` is the fast memory of the instance (shared memory on the GPU), `gbase` an
-// optional per-instance slab of global memory (L2).  LEVEL 0: everything in `base`; LEVEL 1: the Riccati
-// gains and the box slacks / multipliers move to `gbase`; LEVEL 2: also the stage Hessian / gradient /
-// Newton step arrays.  With hinge_arrays = false the per-hinge arrays (hx, hy, hc: caller; hs, hnu: first
-// in `gbase`) are left out of `base` (each entry is touched only by the lane that owns its stage).
-// LEVEL is a compile-time constant so that every pointer keeps a single provenance (the compiler then
-// emits LDS / LDG instead of generic loads).  Returns the bytes of `base` used; *gbytes the bytes of `gbase`.
-// BSG (with LEVEL 0): only the box slacks / multipliers move to `gbase` — 4.8 KB less shared memory per instance at the
-// metric size (13.2 KB: 16 resident instances per SM instead of 12, if the registers allow it).
-template <typename Real, typename Slk = Real, int LEVEL = 0, bool BSG = false>
-RDA_HD size_t su_work_layout(int T, int N, SuWork<Real, Slk>* w, char* base, bool hinge_arrays = true,
+// optional per-instance slab of global memory (L2).  Everything lives in `base`, except that with
+// hinge_arrays = false the per-hinge arrays (hx, hy, hc: caller; hs, hnu: `gbase`) are left out of it (each
+// entry is touched only by the lane that owns its stage).  Returns the bytes of `base` used; *gbytes the
+// bytes of `gbase`.
+template <typename Real>
+RDA_HD size_t su_work_layout(int T, int N, SuWork<Real>* w, char* base, bool hinge_arrays = true,
                              char* gbase = nullptr, size_t* gbytes = nullptr) {
   size_t offs = 0, offg = 0;
   auto takes = [&](size_t n, size_t elt) {
@@ -115,7 +90,6 @@ RDA_HD size_t su_work_layout(int T, int N, SuWork<Real, Slk>* w, char* base, boo
   };
 #define RDA_TAKE_S(field, n, type) { char* p_ = takes((size_t)(n), sizeof(type)); if (w) w->field = (type*)p_; }
 #define RDA_TAKE_G(field, n, type) { char* p_ = takeg((size_t)(n), sizeof(type)); if (w) w->field = (type*)p_; }
-#define RDA_TAKE_L(lv, field, n, type) { if (LEVEL >= (lv)) RDA_TAKE_G(field, n, type) else RDA_TAKE_S(field, n, type) }
   RDA_TAKE_S(s, 3 * (T + 1), Real) RDA_TAKE_S(u, 2 * T, Real) RDA_TAKE_S(d, T, Real)
   RDA_TAKE_S(ref, 3 * (T + 1), float) RDA_TAKE_S(lins, 3 * (T + 1), float)
   RDA_TAKE_S(Aj, 2 * T, Real) RDA_TAKE_S(Bj, 6 * T, Real)
@@ -123,29 +97,28 @@ RDA_HD size_t su_work_layout(int T, int N, SuWork<Real, Slk>* w, char* base, boo
   RDA_TAKE_S(hmask, T * ((N + 31) / 32 > 0 ? (N + 31) / 32 : 1), unsigned)
   if (hinge_arrays) {
     RDA_TAKE_S(hx, N * T, float) RDA_TAKE_S(hy, N * T, float) RDA_TAKE_S(hc, N * T, float)
-    RDA_TAKE_S(hs, N * T, Slk) RDA_TAKE_S(hnu, N * T, Slk)
+    RDA_TAKE_S(hs, N * T, Real) RDA_TAKE_S(hnu, N * T, Real)
   } else {
-    RDA_TAKE_G(hs, N * T, Slk) RDA_TAKE_G(hnu, N * T, Slk)
+    RDA_TAKE_G(hs, N * T, Real) RDA_TAKE_G(hnu, N * T, Real)
   }
-  if (LEVEL >= 1 || BSG) { RDA_TAKE_G(bs, 10 * T, Slk) RDA_TAKE_G(bnu, 10 * T, Slk) } else { RDA_TAKE_S(bs, 10 * T, Slk) RDA_TAKE_S(bnu, 10 * T, Slk) }
-  RDA_TAKE_L(2, Wm, 8 * T + 5, Real)                                  // (Wm, wb) | (dza, dva)
+  RDA_TAKE_S(bs, 10 * T, Real) RDA_TAKE_S(bnu, 10 * T, Real)
+  RDA_TAKE_S(Wm, 8 * T + 5, Real)                                     // (Wm, wb) | (dza, dva)
   if (w) { w->wb = w->Wm + 3 * T; w->dza = w->Wm; w->dva = w->Wm + 5 * (T + 1); }
-  RDA_TAKE_L(2, Ed, 3 * T, Real) RDA_TAKE_L(2, g5q, T, Real)
-  RDA_TAKE_L(2, gw, 8 * T + 5, Real)                                  // gw | (dz, dv)
+  RDA_TAKE_S(Ed, 3 * T, Real) RDA_TAKE_S(g5q, T, Real)
+  RDA_TAKE_S(gw, 8 * T + 5, Real)                                     // gw | (dz, dv)
   if (w) { w->dz = w->gw; w->dv = w->gw + 5 * (T + 1); }
-  RDA_TAKE_L(1, K, 10 * T, Real) RDA_TAKE_L(1, Lc, 3 * T, Real) RDA_TAKE_L(1, kf, 2 * T, Real)
+  RDA_TAKE_S(K, 10 * T, Real) RDA_TAKE_S(Lc, 3 * T, Real) RDA_TAKE_S(kf, 2 * T, Real)
   if (w) { w->Cj = w->K; w->linu = (float*)w->dv; }
 #undef RDA_TAKE_S
 #undef RDA_TAKE_G
-#undef RDA_TAKE_L
   if (gbytes) *gbytes = (offg + 15) & ~(size_t)15;
   return (offs + 15) & ~(size_t)15;
 }
 
 // size-only query of su_work_layout
-template <typename Real, typename Slk = Real, int LEVEL = 0, bool BSG = false>
+template <typename Real>
 RDA_HD size_t su_work_bytes(int T, int N, bool hinge_arrays = true, size_t* gbytes = nullptr) {
-  return su_work_layout<Real, Slk, LEVEL, BSG>(T, N, (SuWork<Real, Slk>*)nullptr, nullptr, hinge_arrays, nullptr, gbytes);
+  return su_work_layout<Real>(T, N, (SuWork<Real>*)nullptr, nullptr, hinge_arrays, nullptr, gbytes);
 }
 
 // Jacobians of the discrete model about (s, u): linear_ackermann_model :949-963,
@@ -184,8 +157,8 @@ RDA_HD void su_linearise(const SuParams& P, const Real* st, const Real* ut, Real
 template <typename Real>
 struct Row { Real g; Real sgn; int comp; bool rate; bool live; };
 
-template <typename Real, typename Slk>
-RDA_HD Row<Real> su_row(const SuParams& P, const SuWork<Real, Slk>& W, int t, int c) {
+template <typename Real>
+RDA_HD Row<Real> su_row(const SuParams& P, const SuWork<Real>& W, int t, int c) {
   Row<Real> r;
   r.rate = c >= 6;
   r.live = true;
@@ -220,8 +193,8 @@ RDA_HD Real su_row_dir(const Row<Real>& r, const Real* dz_t, const Real* dv_t) {
   return r.sgn * x;
 }
 
-template <typename Real, typename Slk, typename Ctx>
-RDA_HD void su_riccati(const SuParams& P, SuWork<Real, Slk>& W, Ctx& ctx, bool factor, Real* dz, Real* dv) {
+template <typename Real, typename Ctx>
+RDA_HD void su_riccati(const SuParams& P, SuWork<Real>& W, Ctx& ctx, bool factor, Real* dz, Real* dv) {
   // Riccati recursion of the Newton step (banded KKT system).  Stage t: state z = (s_t, u_{t-1}),
   // control v = u_t.  The safety distance d_t appears in stage t only (hinges and its own bounds), so
   // it has been eliminated from the stage cost by the assembly (Schur complement on Q_dd: W.Wm holds
@@ -353,8 +326,8 @@ RDA_HD void su_riccati(const SuParams& P, SuWork<Real, Slk>& W, Ctx& ctx, bool f
 // are computed here from (gx, gy) planes passed as pointers (global or shared memory, [o*T+t]).
 // On entry W.d holds para_dis (initial guess of d).  Returns 0 (converged), 1 (iteration cap),
 // 2 (non-finite).  On return W.s, W.u, W.d hold the solution.
-template <typename Real, typename Slk, typename Ctx>
-RDA_HD int su_solve(const SuParams& P, SuWork<Real, Slk>& W, Ctx& ctx, const float* gx, const float* gy,
+template <typename Real, typename Ctx>
+RDA_HD int su_solve(const SuParams& P, SuWork<Real>& W, Ctx& ctx, const float* gx, const float* gy,
                     int* iters_out) {
   const int T = P.T, N = P.N;
   const int lane = ctx.lane(), nl = ctx.nlanes();
@@ -410,10 +383,10 @@ RDA_HD int su_solve(const SuParams& P, SuWork<Real, Slk>& W, Ctx& ctx, const flo
   int nrows = 0;
   for (int t = lane; t < T; t += nl) {
     _Pragma("unroll 1") for (int c = 0; c < 10; ++c) {
-      Row<Real> r = su_row<Real, Slk>(P, W, t, c);
+      Row<Real> r = su_row<Real>(P, W, t, c);
       Real sv = r.live ? rmax(r.g, (Real)1e-2) : (Real)1;
-      W.bs[RDA_SU_BSI(T, t, c)] = sv;
-      W.bnu[RDA_SU_BSI(T, t, c)] = r.live ? mu0 / sv : (Real)0;
+      W.bs[10 * t + c] = sv;
+      W.bnu[10 * t + c] = r.live ? mu0 / sv : (Real)0;
       if (r.live) ++nrows;
     }
     if (acc) {
@@ -478,9 +451,9 @@ RDA_HD int su_solve(const SuParams& P, SuWork<Real, Slk>& W, Ctx& ctx, const flo
         gw[6] = 0; gw[7] = 0;
         Real wb[5] = {0, 0, 0, 0, 0};
         _Pragma("unroll 1") for (int c = 0; c < 10; ++c) {
-          Row<Real> r = su_row<Real, Slk>(P, W, t, c);
+          Row<Real> r = su_row<Real>(P, W, t, c);
           if (!r.live) continue;
-          Real sv = W.bs[RDA_SU_BSI(T, t, c)], nu = W.bnu[RDA_SU_BSI(T, t, c)];
+          Real sv = W.bs[10 * t + c], nu = W.bnu[10 * t + c];
           Real res = r.g - sv;
           const Real isv = rcp_(sv);
           Real om = nu * isv;
@@ -578,16 +551,16 @@ RDA_HD int su_solve(const SuParams& P, SuWork<Real, Slk>& W, Ctx& ctx, const flo
         if (mu < tol_mu && rmx < tol_r && (last_step < tol_step || mu < tol_floor)) { status = 0; break; }
       }
       ctx.sync();
-      su_riccati<Real, Slk, Ctx>(P, W, ctx, phase == 0, phase == 0 ? W.dza : W.dz, phase == 0 ? W.dva : W.dv);
+      su_riccati<Real, Ctx>(P, W, ctx, phase == 0, phase == 0 ? W.dza : W.dz, phase == 0 ? W.dva : W.dv);
       // ---- step lengths ----
       const Real* dz = phase == 0 ? W.dza : W.dz;
       const Real* dv = phase == 0 ? W.dva : W.dv;
       Real rmaxr = 0, s0 = 0, s1 = 0, s2 = 0;   // rmaxr = max over rows of (-delta / value): 1 / max step
       for (int t = lane; t < T; t += nl) {
         _Pragma("unroll 1") for (int c = 0; c < 10; ++c) {
-          Row<Real> r = su_row<Real, Slk>(P, W, t, c);
+          Row<Real> r = su_row<Real>(P, W, t, c);
           if (!r.live) continue;
-          Real sv = W.bs[RDA_SU_BSI(T, t, c)], nu = W.bnu[RDA_SU_BSI(T, t, c)];
+          Real sv = W.bs[10 * t + c], nu = W.bnu[10 * t + c];
           Real res = r.g - sv;
           Real dir = su_row_dir<Real>(r, dz + 5 * t, dv + 3 * t);
           Real ds = dir + res, dn;
@@ -654,10 +627,8 @@ RDA_HD int su_solve(const SuParams& P, SuWork<Real, Slk>& W, Ctx& ctx, const flo
         sg = sg * sg * sg;
         sigma_mu = rmin(sg, (Real)1) * mu;
       } else {
-        // fraction to the boundary (RDA_SU_TAU_ADAPT above; the adaptive rule is an experiment knob, float64 only)
-        const Real tau_b = ((RDA_SU_TAU_ADAPT) > 0 && sizeof(Real) == 8)
-                               ? rmax((Real)0.995, (Real)1 - (Real)(RDA_SU_TAU_ADAPT) * mu) : (Real)0.995;
-        Real a = rmin((Real)1, tau_b * amax);
+        // fixed fraction to the boundary: an adaptive one saved iterations but cycled on a box-only problem (DESIGN.md §4)
+        Real a = rmin((Real)1, (Real)0.995 * amax);
 #ifdef RDA_SU_DEBUG
         printf("   alpha %.3e sigma_mu %.3e\n", (double)a, (double)sigma_mu);
 #endif
@@ -665,11 +636,11 @@ RDA_HD int su_solve(const SuParams& P, SuWork<Real, Slk>& W, Ctx& ctx, const flo
         for (int t = lane; t < T; t += nl) {
           // rows first: they read the OLD iterate through su_row
           Real gsave[10];
-          _Pragma("unroll 1") for (int c = 0; c < 10; ++c) { Row<Real> r = su_row<Real, Slk>(P, W, t, c); gsave[c] = r.g; }
+          _Pragma("unroll 1") for (int c = 0; c < 10; ++c) { Row<Real> r = su_row<Real>(P, W, t, c); gsave[c] = r.g; }
           _Pragma("unroll 1") for (int c = 0; c < 10; ++c) {
-            Row<Real> r = su_row<Real, Slk>(P, W, t, c);
+            Row<Real> r = su_row<Real>(P, W, t, c);
             if (!r.live) continue;
-            Real sv = W.bs[RDA_SU_BSI(T, t, c)], nu = W.bnu[RDA_SU_BSI(T, t, c)];
+            Real sv = W.bs[10 * t + c], nu = W.bnu[10 * t + c];
             Real res = gsave[c] - sv;
             Real dir = su_row_dir<Real>(r, W.dz + 5 * t, W.dv + 3 * t);
             Real ds = dir + res;
@@ -678,8 +649,8 @@ RDA_HD int su_solve(const SuParams& P, SuWork<Real, Slk>& W, Ctx& ctx, const flo
             const Real isv = rcp_(sv), om = nu * isv;
             Real dna = -nu - om * dsa;
             Real dn = (sigma_mu - dsa * dna) * isv - nu - om * ds;
-            W.bs[RDA_SU_BSI(T, t, c)] = sv + a * ds;
-            W.bnu[RDA_SU_BSI(T, t, c)] = nu + a * dn;
+            W.bs[10 * t + c] = sv + a * ds;
+            W.bnu[10 * t + c] = nu + a * dn;
           }
           if (acc) {
             const Real dx = W.s[3 * t + 3] - W.pref[2 * t], dy = W.s[3 * t + 4] - W.pref[2 * t + 1], dd = W.d[t];

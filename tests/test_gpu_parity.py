@@ -353,40 +353,6 @@ def test_coherent_first_pass_matches_the_search_pass(monkeypatch):
     assert float(du.median()) < 2e-5 and float(du.max()) < 3 * TRAJ_TOL
 
 
-@pytest.mark.parametrize('split', [False, True])
-def test_batched_su_pipeline_equals_one_warp_per_instance(monkeypatch, split):
-    """Large sub-batches run the su-QP as a pipeline of wide kernels (su_batched.cuh) instead of k_su.  Forced
-    here on a small batch (RDA_B200_SU_BATCHED=1): trajectories and persistent state must agree with the
-    one-warp-per-instance kernel to float32 rounding, also across the two-stream split and a warm-started call."""
-    from rda_planner_b200.rda_solver import RDA_solver
-    from rda_planner_b200 import _cabi
-    T, N, B = 16, 8, 70
-    car = rectangle_robot()
-    insts, inp = _batch_inputs(B, T, N, 2500, lateral=(0.3, 3.5))
-    dev = {k: torch.as_tensor(v, device='cuda', dtype=torch.int32 if 'kind' in k or 'count' in k else torch.float32)
-           for k, v in inp.items()}
-    monkeypatch.setenv('RDA_B200_SPLIT_MIN', '2' if split else '1000000')
-    monkeypatch.setenv('RDA_B200_SMALL', '0')
-    monkeypatch.setenv('RDA_B200_SU_PRUNE', '0')       # the pipeline keeps every hinge: compare like with like
-    res = {}
-    for mode in ('0', '1'):
-        monkeypatch.setenv('RDA_B200_SU_BATCHED', mode)
-        g = RDA_solver(T, car, 4, N, iter_num=6, iter_threshold=0.0, time_print=False, batch=B)
-        out = {k: v.clone() for k, v in g.iterative_solve_batch(**dev, time_varying=False).items()}
-        out2 = {k: v.clone() for k, v in g.iterative_solve_batch(**dev, time_varying=False).items()}
-        state = {b: g.state_buffer(b).clone() for b in (_cabi.BUF_LAM, _cabi.BUF_MU, _cabi.BUF_Z, _cabi.BUF_ZETA, _cabi.BUF_DIS)}
-        res[mode] = (out, out2, state, g.launch_count())
-    assert res['1'][3] > 3 * res['0'][3]              # the pipeline really ran
-    for call in (0, 1):
-        a, b = res['0'][call], res['1'][call]
-        assert torch.equal(a['status'] & 6, b['status'] & 6) and int((b['status'] & 6).sum()) == 0
-        assert torch.equal(a['iters'], b['iters'])
-        for k in ('u', 's'):
-            assert float((a[k] - b[k]).abs().max()) < 2e-5, (call, k, float((a[k] - b[k]).abs().max()))
-    for k in res['0'][2]:
-        assert float((res['0'][2][k] - res['1'][2][k]).abs().max()) < 1e-4, k
-
-
 def test_graph_replay_of_the_single_instance_api():
     """RDA_solver(graph=True): the reference-signature call stages its inputs in persistent device buffers and replays
     one CUDA graph per control step; results and warm-start evolution must be bit-identical to eager launches."""

@@ -166,14 +166,37 @@ def test_su_core_is_closer_to_the_optimum_than_a_1e9_oracle_solve_at_metric_size
     assert loose[0] > 3 * core[0] and loose[1] > 3 * core[1]
 
 
+def _params(T, N, dyn='acker', acc=1):
+    return shim.SuParams(T=T, N=N, dynamics=shim.DYN[dyn], accelerated=acc, dt=0.1, L=3.0,
+                         umax=(shim.C.c_float * 2)(10, 1), ab=(shim.C.c_float * 2)(1.0, 0.05), ws=1, wu=1, slack_gain=8,
+                         dmin=0.1, dmax=1.0, ro1=200, ro2=1, max_iter=40, mu0=1.0)
+
+
+def _inputs(nb, T, N, dyn, seed):
+    """nb su-QPs with hinge rows that are partly active: unit normals, margins in [-0.5, 3]."""
+    rng = np.random.default_rng(seed)
+    cur_s = np.zeros((nb, 3, T + 1), np.float32); cur_u = np.zeros((nb, 2, T), np.float32)
+    ref_s = np.zeros((nb, 3, T + 1), np.float32); pref = np.zeros((nb, 2, T), np.float32)
+    coef = np.zeros((nb, 5, N, T), np.float32); dis = np.ones((nb, T), np.float32)
+    vref = np.full(nb, 4.0, np.float32)
+    for b in range(nb):
+        inst = make_instance(seed * 100 + b, T=T, N=max(N, 1), E=4, dynamics=dyn, lateral=(0.3, 3.5))
+        cur_s[b] = inst['nom_s']; cur_u[b] = inst['nom_u']; ref_s[b] = inst['ref']
+        pref[b] = inst['nom_s'][0:2, 1:] + rng.normal(0, 0.05, (2, T))
+        ang = rng.uniform(-np.pi, np.pi, (N, T))
+        coef[b, 0] = np.cos(ang); coef[b, 1] = np.sin(ang)
+        coef[b, 2] = rng.uniform(-0.5, 3.0, (N, T))
+        coef[b, 3:5] = rng.normal(0, 0.3, (2, N, T))
+        dis[b] = rng.uniform(0.1, 1.0, T)
+    return cur_s, cur_u, ref_s, pref, coef, dis, vref
+
+
 @pytest.mark.parametrize('dyn,N,seed', [('acker', 0, 7), ('acker', 0, 11), ('diff', 0, 11), ('omni', 0, 11), ('acker', 5, 11),
                                         ('diff', 5, 11), ('omni', 5, 11)])
 def test_su_core_converges_on_random_problems(dyn, N, seed):
-    """Robustness guard of the interior point iteration (third session of round 2: a seemingly harmless change of the fraction
-    to the boundary made it CYCLE on a box-only problem, su_solver.cuh RDA_SU_TAU_ADAPT): 40 random problems per case,
-    without hinges (N = 0: only the control / rate boxes) and with hinges near activity — every solve converges, well below
-    the iteration cap, float64 and float32."""
-    from test_su_batched import _params, _inputs
+    """Robustness guard of the interior point iteration (third session of round 2: an adaptive fraction to the boundary made
+    it CYCLE on a box-only problem, DESIGN.md §4): 40 random problems per case, without hinges (N = 0: only the control /
+    rate boxes) and with hinges near activity — every solve converges, well below the iteration cap, float64 and float32."""
     T, nb = 12, 40
     P = _params(T, N, dyn, 1)
     cur_s, cur_u, ref_s, pref, coef, dis, vref = _inputs(nb, T, N, dyn, seed)       # seed 7 holds the problem that cycled
@@ -188,3 +211,18 @@ def test_su_core_converges_on_random_problems(dyn, N, seed):
             assert np.all(np.isfinite(s)) and np.all(np.isfinite(u))
             worst = max(worst, it)
     assert worst <= 30, worst
+
+
+def test_iteration_cap_is_reported_like_optimal_inaccurate():
+    """A solve stopped by the iteration cap returns status 1 (k_su accepts it, as the reference accepts ECOS'
+    OPTIMAL_INACCURATE) with a finite iterate and every allowed iteration counted."""
+    T, N, nb = 10, 4, 3
+    P = _params(T, N)
+    P.max_iter = 3
+    cur_s, cur_u, ref_s, pref, coef, dis, vref = _inputs(nb, T, N, 'acker', 11)
+    for b in range(nb):
+        for prec in ('d', 'f'):
+            s, u, d, st, it = shim.su(P, cur_s[b].astype(float), cur_u[b].astype(float), ref_s[b].astype(float), float(vref[b]),
+                                      dis[b].astype(float), *coef[b], pref[b].astype(float), prec=prec)
+            assert st == 1 and it == 3, (b, prec, st, it)
+            assert np.all(np.isfinite(s)) and np.all(np.isfinite(u)) and np.all(np.isfinite(d))
