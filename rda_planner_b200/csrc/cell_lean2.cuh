@@ -1,4 +1,4 @@
-// cell_lean2.cuh — coherent first pass of the (lam, mu, z) cell kernel (PREPARED FOR ROUND 2, not launched yet).
+// cell_lean2.cuh — coherent first pass of the (lam, mu, z) cell kernel, run by k_cells_coh (rda_kernels.cu).
 //
 // Same two closed-form cases as cell_lean.cuh (xi = 0, margin >= 0), restricted to clearly separated
 // polygon/polygon cells, but without the search: the closest pair of two convex polygons always involves

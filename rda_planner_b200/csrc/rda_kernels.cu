@@ -431,16 +431,17 @@ __global__ void k_heading(DevPtrs d, float* rot) {
 }
 
 // Coherent first pass (cell_lean2.cuh): one thread per cell tries the support-vertex pair of the previous
-// iteration; what it declines goes to worklist0 and through k_cells_fast<.., LISTED>.  Grid: (cells of one
-// instance / 128, instances) — no 64-bit index arithmetic, one instance per CTA (uniform early exit, one
-// residual atomic per warp), 32-bit offsets inside the instance.
+// iteration; what it declines goes to worklist0 and through k_cells_fast<.., LISTED>.  Grid: one-dimensional,
+// `tiles` = ceil(cells of one instance / 128) CTAs per instance, instance-major (blockIdx.x = b * tiles + tile,
+// so any batch size fits; gridDim.y would cap it at 65 535) — no 64-bit index arithmetic, one instance per CTA
+// (uniform early exit, one residual atomic per warp), 32-bit offsets inside the instance.
 __global__ void __launch_bounds__(128, 6) k_cells_coh(DevPtrs d, RobotGeom rb, RobotAux ra, const float* __restrict__ rot,
-                                                      float theta, float invT) {
+                                                      float theta, float invT, int tiles) {
   constexpr int EC = 4, RC = 4;
   const int T = d.T, N = d.N, E = d.E, R = d.R, NT = N * T;
-  const int b = blockIdx.y;
+  const int b = blockIdx.x / tiles;
   if (d.done[b] || d.obs_count[b] == 0) return;             // uniform for the CTA
-  const int rem = blockIdx.x * blockDim.x + threadIdx.x;
+  const int rem = (blockIdx.x - b * tiles) * blockDim.x + threadIdx.x;
   const int lane = threadIdx.x & 31;
   const bool live = rem < NT;
   float dual = 0.f;
@@ -1453,8 +1454,9 @@ static int step_lammuz_part(rda_handle* h, int b0, int nb, int part, cudaStream_
     if (h->lean2 && !h->obs_tv && h->E <= 4 && h->R <= 4) {
       k_heading<<<(nb * h->T + 255) / 256, 256, 0, s>>>(d, h->rot + (size_t)b0 * 2 * h->T);
       RDA_CUDA(cudaGetLastError());
-      k_cells_coh<<<dim3((h->N * h->T + 127) / 128, nb), 128, 0, s>>>(d, h->rb, h->ra, h->rot + (size_t)b0 * 2 * h->T, theta,
-                                                                       1.0f / (float)h->T);
+      const int tiles = (h->N * h->T + 127) / 128;
+      k_cells_coh<<<(unsigned)tiles * (unsigned)nb, 128, 0, s>>>(d, h->rb, h->ra, h->rot + (size_t)b0 * 2 * h->T, theta,
+                                                                1.0f / (float)h->T, tiles);
       h->launches += 1;
       RDA_CUDA(cudaGetLastError());
       k_cells_fast<4, 4, true><<<grid_for((long long)nb * h->N * h->T, 128, h->sms), 128, 0, s>>>(d, h->rb, theta);
