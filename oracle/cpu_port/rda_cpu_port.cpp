@@ -237,7 +237,7 @@ extern "C" int port_solve_batch(const rda_config* cfg, const rda_tunables* tun, 
     RobotAux ra2;
     robot_aux_from_geom(rb, &ra2);
     long long coh_hits = 0;
-    if (use_lean2 && E == 4 && !tv && !rb.disc)
+    if (use_lean2 && E <= 4 && R <= 4 && !tv && !rb.disc)
       for (int o = 0; o < N; ++o) obstacle_geometry<4>(E, obs_A + ((size_t)b * N + o) * E * 2, obs_b + ((size_t)b * N + o) * E, og2[o]);
     std::vector<float> cs(nom_s + (size_t)b * 3 * (T + 1), nom_s + (size_t)(b + 1) * 3 * (T + 1));
     std::vector<float> cu(nom_u + (size_t)b * 2 * T, nom_u + (size_t)(b + 1) * 2 * T);
@@ -294,9 +294,10 @@ extern "C" int port_solve_batch(const rda_config* cfg, const rda_tunables* tun, 
             }
 #endif
             CellOut<float> out;
-            // emulation of the coherent pipeline (RDA_PORT_LEAN2=1): k_cells_coh -> listed cell_lean -> generic solver
+            // emulation of the coherent pipeline (RDA_PORT_LEAN2=1): k_cells_coh -> listed cell_lean -> generic solver, under the
+            // library's condition (rda_create / step_lammuz_part: E <= 4, R <= 4, static polygons; padded rows are zero)
             bool lean_done = false;
-            if (use_lean2 && !rb.disc && E == 4 && R == 4 && !tv && obs_kind[(size_t)b * N + o] == RDA_OBS_POLYGON) {
+            if (use_lean2 && !rb.disc && E <= 4 && R <= 4 && !tv && obs_kind[(size_t)b * N + o] == RDA_OBS_POLYGON) {
               LeanOut<4, 4> lo;
               int nf = -1;
               if (xi[o * T + t] == 0.f && xi[NT + o * T + t] == 0.f)
