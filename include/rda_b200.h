@@ -138,7 +138,7 @@ const char *rda_version(void);
 
 /* MPC.pre_process (mpc.py:251-291) with closest_point :338-353, inter_point :355-383,
  * range_cir_seg :385-423, wraptopi :431-438 and motion_predict_model_* :293-336, for B
- * robots on ONE reference path.
+ * robots on ONE reference path (rda_pre_process_paths below lets each robot follow its own).
  *   state [B][3]; cur_vel [B][2][T] (the controls of the previous step, MPC.cur_vel_array);
  *   ref_speed [B] (already multiplied by the gear); path [P][3] (x, y, heading);
  *   start_index [B] (MPC.cur_index; NULL = 0); threshold / ind_range: closest_point kwargs
@@ -208,6 +208,37 @@ int rda_pre_process_curves(int B, int T, int dynamics, float dt, float wheelbase
 int rda_post_process_gear(int B, int T, int n_curves, const int32_t *curve_start, int goal_index_threshold,
                           int32_t *near_index, int32_t *curve_index, float *u_opt, float *cur_vel,
                           int32_t *arrive, void *cuda_stream);
+
+/* A FLEET on its own reference paths: each robot follows its own path, picked from a shared set of W paths, as
+ * a batch of reference MPC objects each owning its ref_path (mpc.py:67-125, update_ref_path :220-227).  The
+ * rda_pre_process / rda_pre_process_curves / rda_post_process / rda_post_process_gear calls above are the W = 1
+ * case of these two.
+ *   path [P][3]: the waypoints of all paths, one flat list; every path is cut into single-gear curves
+ *   (split_path, mpc.py:232-249; without enable_reverse a path is one curve of gear +1):
+ *   path_curve [W+1]: path w is curves [path_curve[w], path_curve[w+1]);
+ *   curve_start [C+1]: curve c is waypoints [curve_start[c], curve_start[c+1]) of `path`;
+ *   curve_gear [C]: +1 forward, -1 reverse;
+ *   robot_path [B]: the path of each robot (NULL: all on path 0);
+ *   curve_index [B]: the robot's curve, relative to its path (NULL: 0; out of range: clamped into the path);
+ *   start_index / near_index [B]: MPC.cur_index, relative to the robot's curve (start_index NULL: 0).
+ * rda_pre_process_paths is rda_pre_process on each robot's curve; solver_speed [B] (may be NULL) receives the
+ * solver's reference speed gear * ref_speed (mpc.py:161).  rda_post_process_paths applies mpc.py:166-185: at the
+ * end of a curve that is not its path's last, the robot moves to the next curve (near_index 0, controls kept);
+ * past its path's last curve the controls are zeroed and arrive is set, and curve_index stays on that last curve.
+ * cur_vel (may be NULL) receives the controls kept; arrive may be NULL.
+ * A robot whose robot_path is outside [0, W), or whose path has no curve, has NO PATH (decided on the device, so
+ * that the host never reads robot_path): nom_s is its rollout as usual, every column of ref_s is its current state,
+ * near_index is 0 and its gear +1; rda_post_process_paths then zeroes its controls and sets arrive.           */
+int rda_pre_process_paths(int B, int T, int dynamics, float dt, float wheelbase, const float *state,
+                          const float *cur_vel, const float *ref_speed, const float *path, int W,
+                          const int32_t *path_curve, const int32_t *curve_start, const int32_t *curve_gear,
+                          const int32_t *robot_path, const int32_t *curve_index, const int32_t *start_index,
+                          float threshold, int ind_range, float *nom_s, float *ref_s, int32_t *near_index,
+                          float *solver_speed, void *cuda_stream);
+int rda_post_process_paths(int B, int T, int W, const int32_t *path_curve, const int32_t *curve_start,
+                           const int32_t *robot_path, int goal_index_threshold, int32_t *near_index,
+                           int32_t *curve_index, float *u_opt, float *cur_vel, int32_t *arrive,
+                           void *cuda_stream);
 
 /* state [B][3] advanced in place by one step of the nonlinear model with the first control of
  * u_opt [B][2][T] (mpc.py:293-336; what the examples' simulator does between control calls). */

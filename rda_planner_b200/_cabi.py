@@ -47,7 +47,8 @@ EXPORTS = ['rda_create', 'rda_destroy', 'rda_set_tunables', 'rda_get_tunables', 
            'rda_cold_start', 'rda_solve', 'rda_begin', 'rda_step_su', 'rda_step_lammuz', 'rda_finish',
            'rda_get_buffer', 'rda_copy_buffer', 'rda_last_launch_count', 'rda_version',
            'rda_pre_process', 'rda_convert_obstacles', 'rda_post_process', 'rda_motion_predict',
-           'rda_pre_process_curves', 'rda_post_process_gear', 'rda_convert_world_obstacles']
+           'rda_pre_process_curves', 'rda_post_process_gear', 'rda_convert_world_obstacles',
+           'rda_pre_process_paths', 'rda_post_process_paths']
 MAX_SHAPES = 64
 MAX_WORLD_SLOTS = 256
 
@@ -88,6 +89,9 @@ def load():
     lib.rda_post_process.argtypes = [i, i, i, i, vp, vp, vp, vp, vp]
     lib.rda_pre_process_curves.argtypes = [i, i, i, f, f, vp, vp, vp, vp, i, vp, vp, vp, f, i, vp, vp, vp, vp]
     lib.rda_post_process_gear.argtypes = [i, i, i, vp, i, vp, vp, vp, vp, vp, vp]
+    lib.rda_pre_process_paths.argtypes = [i, i, i, f, f, vp, vp, vp, vp, i, vp, vp, vp, vp, vp, vp, f, i, vp, vp, vp, vp,
+                                          vp]
+    lib.rda_post_process_paths.argtypes = [i, i, i, vp, vp, vp, i, vp, vp, vp, vp, vp, vp]
     lib.rda_motion_predict.argtypes = [i, i, i, f, f, vp, vp, vp]
     for name in EXPORTS:
         if name != 'rda_version':

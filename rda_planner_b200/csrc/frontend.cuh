@@ -120,6 +120,53 @@ RDA_HD int pre_process_one(int dynamics, int T, double dt, double L, const float
   return near;
 }
 
+// A robot without a reference path: the nominal rollout of pre_process_one, and a reference that holds the robot's
+// current state in every column.
+RDA_HD void hold_state_one(int dynamics, int T, double dt, double L, const float* state, const float* vel,
+                           float* nom_s, float* ref_s) {
+  const int S = T + 1;
+  double cur[3] = {state[0], state[1], state[2]};
+  for (int r = 0; r < 3; ++r) {
+    nom_s[r * S] = state[r];
+    for (int j = 0; j < S; ++j) ref_s[r * S + j] = state[r];
+  }
+  for (int i = 0; i < T; ++i) {
+    double nxt[3];
+    motion_predict(dynamics, dt, L, cur, vel[i], vel[T + i], nxt);
+    for (int r = 0; r < 3; ++r) { cur[r] = nxt[r]; nom_s[r * S + i + 1] = (float)cur[r]; }
+  }
+}
+
+// ---- reference path sets ----------------------------------------------------------------------
+// W paths in one flat waypoint list path [P][3], each cut into single-gear curves (split_path, mpc.py:232-249):
+// path w is curves [path_curve[w], path_curve[w+1]), curve c is waypoints [curve_start[c], curve_start[c+1]) with
+// gear curve_gear[c] (+1 / -1).  NULL tables describe a single path: path_curve NULL = one path of n_curves
+// curves, curve_start NULL = one curve of P waypoints, curve_gear NULL = gear +1.
+struct PathCurve {
+  int index;   // curve index relative to the path, clamped into [0, count)
+  int count;   // curves of the path
+  int first;   // first waypoint of the curve in the flat list
+  int len;     // waypoints of the curve
+  int gear;    // +1 forward, -1 reverse
+};
+
+// The curve a robot on path w (0 <= w < W) with relative curve index c follows.  Out-of-range c is clamped to the
+// path's first or last curve.  Returns false for a path without curves.
+RDA_HD bool resolve_curve(int w, int c, const int* path_curve, int n_curves, const int* curve_start, int P,
+                          const int* curve_gear, PathCurve* out) {
+  const int c0 = path_curve ? path_curve[w] : 0;
+  const int nc = path_curve ? path_curve[w + 1] - c0 : n_curves;
+  if (nc < 1) return false;
+  c = c < 0 ? 0 : (c >= nc ? nc - 1 : c);
+  const int g = c0 + c;
+  out->index = c;
+  out->count = nc;
+  out->first = curve_start ? curve_start[g] : 0;
+  out->len = curve_start ? curve_start[g + 1] - out->first : P;
+  out->gear = curve_gear ? curve_gear[g] : 1;
+  return true;
+}
+
 // ---- obstacles ------------------------------------------------------------------------------
 // One raw shape: kind RDA_OBS_POLYGON (nv vertices xy[2 i], xy[2 i + 1]) or RDA_OBS_CIRCLE (centre xy[0..1],
 // radius), constant velocity (vx, vy).

@@ -15,33 +15,34 @@ using namespace rda;
 
 namespace {
 
-__global__ void k_pre_process(int B, int T, int dynamics, float dt, float L, const float* state, const float* cur_vel,
-                              const float* ref_speed, const float* path, int P, const int* start_index,
-                              float threshold, int ind_range, float* nom_s, float* ref_s, int* near_index) {
+// MPC.pre_process on the single-gear curve each robot follows (mpc.py:139-144, :251-291), and the solver's reference
+// speed gear * ref_speed (mpc.py:161).  A robot whose path index is outside [0, W) has no path: its nominal rollout as
+// usual, a reference that holds its current state, near_index 0 and gear +1.
+__global__ void k_pre_process_paths(int B, int T, int dynamics, float dt, float L, const float* state,
+                                    const float* cur_vel, const float* ref_speed, const float* path, int P, int W,
+                                    int n_curves, const int* path_curve, const int* curve_start, const int* curve_gear,
+                                    const int* robot_path, const int* curve_index, const int* start_index,
+                                    float threshold, int ind_range, float* nom_s, float* ref_s, int* near_index,
+                                    float* solver_speed) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
-  const int near = pre_process_one(dynamics, T, (double)dt, (double)L, state + 3 * (size_t)b,
-                                   cur_vel + (size_t)b * 2 * T, (double)ref_speed[b], path, P,
-                                   start_index ? start_index[b] : 0, (double)threshold, ind_range,
-                                   nom_s + (size_t)b * 3 * (T + 1), ref_s + (size_t)b * 3 * (T + 1));
+  const int w = robot_path ? robot_path[b] : 0;
+  const float* st = state + 3 * (size_t)b;
+  const float* vel = cur_vel + (size_t)b * 2 * T;
+  float* nom = nom_s + (size_t)b * 3 * (T + 1);
+  float* ref = ref_s + (size_t)b * 3 * (T + 1);
+  PathCurve cv;
+  int near = 0, gear = 1;
+  if (w >= 0 && w < W &&
+      resolve_curve(w, curve_index ? curve_index[b] : 0, path_curve, n_curves, curve_start, P, curve_gear, &cv)) {
+    near = pre_process_one(dynamics, T, (double)dt, (double)L, st, vel, (double)ref_speed[b], path + 3 * (size_t)cv.first,
+                           cv.len, start_index ? start_index[b] : 0, (double)threshold, ind_range, nom, ref);
+    gear = cv.gear;
+  } else {
+    hold_state_one(dynamics, T, (double)dt, (double)L, st, vel, nom, ref);
+  }
   near_index[b] = near;
-}
-
-// the same on the single-gear curve the robot currently follows (enable_reverse, mpc.py:139-144)
-__global__ void k_pre_process_curves(int B, int T, int dynamics, float dt, float L, const float* state, const float* cur_vel,
-                                     const float* ref_speed, const float* path, int n_curves, const int* curve_start,
-                                     const int* curve_index, const int* start_index, float threshold, int ind_range,
-                                     float* nom_s, float* ref_s, int* near_index) {
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= B) return;
-  int c = curve_index[b];
-  c = c < 0 ? 0 : (c >= n_curves ? n_curves - 1 : c);
-  const int p0 = curve_start[c], len = curve_start[c + 1] - p0;
-  const int near = pre_process_one(dynamics, T, (double)dt, (double)L, state + 3 * (size_t)b,
-                                   cur_vel + (size_t)b * 2 * T, (double)ref_speed[b], path + 3 * (size_t)p0, len,
-                                   start_index ? start_index[b] : 0, (double)threshold, ind_range,
-                                   nom_s + (size_t)b * 3 * (T + 1), ref_s + (size_t)b * 3 * (T + 1));
-  near_index[b] = near;
+  if (solver_speed) solver_speed[b] = ref_speed[b] * (float)gear;
 }
 
 // one CTA per instance: keys -> stable ranks -> rows of the N slots
@@ -202,31 +203,26 @@ k_convert_world_obstacles(int B, int W, int N, int T, int E, float dt, int time_
   }
 }
 
-// arrive rule (mpc.py:170-185 without gear changes) and the controls kept as next nominal (mpc.py:186)
-__global__ void k_post_process(int B, int T, int P, int goal_index_threshold, const int* near_index, float* u_opt,
-                               float* cur_vel, int* arrive) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= B * 2 * T) return;
-  const int b = i / (2 * T);
-  const bool arr = near_index[b] >= P - goal_index_threshold;
-  float u = u_opt[i];
-  if (arr) { u = 0.f; u_opt[i] = 0.f; }
-  if (cur_vel) cur_vel[i] = u;
-  if (arrive && i == b * 2 * T) arrive[b] = arr ? 1 : 0;
-}
-
-// end-of-curve rule with gear changes (mpc.py:166-185), one thread per robot
-__global__ void k_post_process_gear(int B, int T, int n_curves, const int* curve_start, int goal_index_threshold,
-                                    int* near_index, int* curve_index, float* u_opt, float* cur_vel, int* arrive) {
+// End-of-curve and arrive rules of MPC.control (mpc.py:166-185) on each robot's own curve and path, one thread per
+// robot.  At the end of a curve that is not its path's last the robot moves on to the next curve (cur_index back to 0,
+// controls kept); past its path's last curve, or without a path, its controls are zeroed and arrive is set.  cur_vel
+// (may be NULL) receives the controls kept (mpc.py:186).  near_index and curve_index are only written on a curve
+// switch, which a path of one curve never makes.
+__global__ void k_post_process_paths(int B, int T, int P, int W, int n_curves, const int* path_curve,
+                                     const int* curve_start, const int* robot_path, int goal_index_threshold,
+                                     int* near_index, int* curve_index, float* u_opt, float* cur_vel, int* arrive) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
-  int c = curve_index[b];
-  c = c < 0 ? 0 : (c >= n_curves ? n_curves - 1 : c);
-  const int len = curve_start[c + 1] - curve_start[c];
-  bool arr = false;
-  if (near_index[b] >= len - goal_index_threshold) {
-    if (c + 1 < n_curves) { curve_index[b] = c + 1; near_index[b] = 0; }     // next curve, controls kept
-    else arr = true;                                                            // past the last curve
+  const int w = robot_path ? robot_path[b] : 0;
+  PathCurve cv;
+  bool arr = true;
+  if (w >= 0 && w < W &&
+      resolve_curve(w, curve_index ? curve_index[b] : 0, path_curve, n_curves, curve_start, P, nullptr, &cv)) {
+    arr = false;
+    if (near_index[b] >= cv.len - goal_index_threshold) {
+      if (cv.index + 1 < cv.count) { curve_index[b] = cv.index + 1; near_index[b] = 0; }   // next curve
+      else arr = true;                                                                     // past the last curve
+    }
   }
   float* u = u_opt + (size_t)b * 2 * T;
   for (int i = 0; i < 2 * T; ++i) {
@@ -254,9 +250,9 @@ int rda_pre_process(int B, int T, int dynamics, float dt, float wheelbase, const
                     int ind_range, float* nom_s, float* ref_s, int32_t* near_index, void* stream) {
   if (B < 1 || T < 1 || P < 1 || dynamics < 0 || dynamics > 2) return RDA_E_ARG;
   if (!state || !cur_vel || !ref_speed || !path || !nom_s || !ref_s || !near_index) return RDA_E_ARG;
-  k_pre_process<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(B, T, dynamics, dt, wheelbase, state, cur_vel, ref_speed,
-                                                                   path, P, start_index, threshold, ind_range, nom_s,
-                                                                   ref_s, near_index);
+  k_pre_process_paths<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(
+      B, T, dynamics, dt, wheelbase, state, cur_vel, ref_speed, path, P, 1, 1, nullptr, nullptr, nullptr, nullptr,
+      nullptr, start_index, threshold, ind_range, nom_s, ref_s, near_index, nullptr);
   RDA_CUDA(cudaGetLastError());
   return 0;
 }
@@ -267,10 +263,24 @@ int rda_pre_process_curves(int B, int T, int dynamics, float dt, float wheelbase
                            float* nom_s, float* ref_s, int32_t* near_index, void* stream) {
   if (B < 1 || T < 1 || n_curves < 1 || dynamics < 0 || dynamics > 2) return RDA_E_ARG;
   if (!state || !cur_vel || !ref_speed || !path || !curve_start || !curve_index || !nom_s || !ref_s || !near_index) return RDA_E_ARG;
-  k_pre_process_curves<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(B, T, dynamics, dt, wheelbase, state, cur_vel,
-                                                                          ref_speed, path, n_curves, curve_start, curve_index,
-                                                                          start_index, threshold, ind_range, nom_s, ref_s,
-                                                                          near_index);
+  k_pre_process_paths<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(
+      B, T, dynamics, dt, wheelbase, state, cur_vel, ref_speed, path, 0, 1, n_curves, nullptr, curve_start, nullptr,
+      nullptr, curve_index, start_index, threshold, ind_range, nom_s, ref_s, near_index, nullptr);
+  RDA_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int rda_pre_process_paths(int B, int T, int dynamics, float dt, float wheelbase, const float* state, const float* cur_vel,
+                          const float* ref_speed, const float* path, int W, const int32_t* path_curve,
+                          const int32_t* curve_start, const int32_t* curve_gear, const int32_t* robot_path,
+                          const int32_t* curve_index, const int32_t* start_index, float threshold, int ind_range,
+                          float* nom_s, float* ref_s, int32_t* near_index, float* solver_speed, void* stream) {
+  if (B < 1 || T < 1 || W < 1 || dynamics < 0 || dynamics > 2) return RDA_E_ARG;
+  if (!state || !cur_vel || !ref_speed || !path || !path_curve || !curve_start || !curve_gear) return RDA_E_ARG;
+  if (!nom_s || !ref_s || !near_index) return RDA_E_ARG;
+  k_pre_process_paths<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(
+      B, T, dynamics, dt, wheelbase, state, cur_vel, ref_speed, path, 0, W, 0, path_curve, curve_start, curve_gear,
+      robot_path, curve_index, start_index, threshold, ind_range, nom_s, ref_s, near_index, solver_speed);
   RDA_CUDA(cudaGetLastError());
   return 0;
 }
@@ -279,8 +289,20 @@ int rda_post_process_gear(int B, int T, int n_curves, const int32_t* curve_start
                           int32_t* near_index, int32_t* curve_index, float* u_opt, float* cur_vel, int32_t* arrive,
                           void* stream) {
   if (B < 1 || T < 1 || n_curves < 1 || !curve_start || !near_index || !curve_index || !u_opt) return RDA_E_ARG;
-  k_post_process_gear<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(B, T, n_curves, curve_start, goal_index_threshold,
-                                                                         near_index, curve_index, u_opt, cur_vel, arrive);
+  k_post_process_paths<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(
+      B, T, 0, 1, n_curves, nullptr, curve_start, nullptr, goal_index_threshold, near_index, curve_index, u_opt, cur_vel,
+      arrive);
+  RDA_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int rda_post_process_paths(int B, int T, int W, const int32_t* path_curve, const int32_t* curve_start,
+                           const int32_t* robot_path, int goal_index_threshold, int32_t* near_index,
+                           int32_t* curve_index, float* u_opt, float* cur_vel, int32_t* arrive, void* stream) {
+  if (B < 1 || T < 1 || W < 1 || !path_curve || !curve_start || !near_index || !curve_index || !u_opt) return RDA_E_ARG;
+  k_post_process_paths<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(
+      B, T, 0, W, 0, path_curve, curve_start, robot_path, goal_index_threshold, near_index, curve_index, u_opt, cur_vel,
+      arrive);
   RDA_CUDA(cudaGetLastError());
   return 0;
 }
@@ -320,9 +342,10 @@ int rda_convert_world_obstacles(int B, int W, int N, int T, int E, float dt, int
 int rda_post_process(int B, int T, int P, int goal_index_threshold, const int32_t* near_index, float* u_opt,
                      float* cur_vel, int32_t* arrive, void* stream) {
   if (B < 1 || T < 1 || !near_index || !u_opt) return RDA_E_ARG;
-  const int n = B * 2 * T;
-  k_post_process<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(B, T, P, goal_index_threshold, near_index, u_opt,
-                                                                    cur_vel, arrive);
+  // one curve of P waypoints: the kernel never switches curves, so near_index is only read
+  k_post_process_paths<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(
+      B, T, P, 1, 1, nullptr, nullptr, nullptr, goal_index_threshold, const_cast<int32_t*>(near_index), nullptr, u_opt,
+      cur_vel, arrive);
   RDA_CUDA(cudaGetLastError());
   return 0;
 }

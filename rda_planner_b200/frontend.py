@@ -6,8 +6,10 @@
   convert_world_obstacles_batch
                            the same over obstacle worlds of any size shared by many robots: each
                            robot's N nearest shapes of its world
-  BatchedMPC               MPC.control for B robots on one reference path (mpc.py:127-187),
-                           closed loop without a host round trip
+  pack_paths               a set of reference paths cut into single-gear curves (split_path, mpc.py:232-249),
+                           in the layout the device reads
+  BatchedMPC               MPC.control for B robots, on one reference path or each on its own path of a
+                           shared set (mpc.py:127-187), closed loop without a host round trip
 
 Thin wrappers over the C ABI (include/rda_b200.h, "front end"); no CPU fallback."""
 import ctypes as C
@@ -36,6 +38,50 @@ def path_tensor(ref_path, device):
     else:
         arr = np.asarray(ref_path, float)[:, :3]
     return torch.as_tensor(arr, dtype=torch.float32, device=device).contiguous()
+
+
+def _path_rows(ref_path):
+    """A reference path in any form path_tensor accepts -> float64 array [P, k], one waypoint per row with all its
+    rows (x, y, heading and, when present, the gear flag)."""
+    if isinstance(ref_path, torch.Tensor):
+        return ref_path.detach().to('cpu', torch.float64).numpy().reshape(len(ref_path), -1)
+    if isinstance(ref_path, (list, tuple)):
+        if not ref_path:
+            return np.zeros((0, 3))
+        return np.stack([np.asarray(p, float).reshape(-1) for p in ref_path])
+    return np.asarray(ref_path, float).reshape(len(ref_path), -1)
+
+
+def pack_paths(paths, enable_reverse=False):
+    """W reference paths, each in any form path_tensor accepts, -> dict of host arrays in the layout of
+    rda_pre_process_paths: path [P,3] float32 (all waypoints, one flat list), curve_start [C+1], path_curve [W+1] and
+    curve_gear [C] int32.  Each path is cut into single-gear curves as split_path does it (mpc.py:232-249): with
+    enable_reverse a new curve starts wherever the gear flag, the last row of a waypoint, changes; without it every
+    path is one curve of gear +1."""
+    rows = [_path_rows(p) for p in paths]
+    if not rows:
+        raise ValueError('at least one path')
+    curve_start, path_curve, gears = [0], [0], []
+    for w, r in enumerate(rows):
+        if len(r) == 0 or r.shape[1] < 3:
+            raise ValueError(f'path {w} is empty or has fewer than 3 rows per waypoint')
+        if enable_reverse:
+            if r.shape[1] < 4:
+                raise ValueError(f'path {w} has no gear row (enable_reverse reads the last of 4 rows)')
+            flags = r[:, -1]
+            cuts = [i for i in range(1, len(r)) if flags[i] != flags[i - 1]]
+        else:
+            flags, cuts = np.ones(len(r)), []
+        base = curve_start[-1]
+        for c in cuts + [len(r)]:
+            curve_start.append(base + c)
+        gears += [int(flags[c]) for c in [0] + cuts]
+        path_curve.append(len(gears))
+    if curve_start[-1] > np.iinfo(np.int32).max:
+        raise ValueError('more than 2**31 - 1 waypoints')
+    return {'path': np.concatenate([r[:, :3] for r in rows]).astype(np.float32),
+            'curve_start': np.asarray(curve_start, np.int32), 'path_curve': np.asarray(path_curve, np.int32),
+            'curve_gear': np.asarray(gears, np.int32)}
 
 
 def _shape_arrays(*lead):
@@ -168,16 +214,20 @@ def shapes_to_device(shapes, device):
 
 
 class BatchedMPC:
-    """MPC.control (mpc.py:127-187) for `batch` robots that follow one reference path, every step on
-    the device: pre_process -> obstacle conversion -> ADMM solve -> arrive rule.  Keyword set of the
-    reference's MPC where it applies.  With `enable_reverse` the path carries a gear flag in its 4th row
-    (+1 forward, -1 reverse; mpc.py:139-144): it is cut into single-gear curves (split_path, mpc.py:232-249),
-    every robot follows its own curve, the solver's reference speed carries the gear's sign and a robot moves on
-    to the next curve when it reaches the end of the current one (mpc.py:166-183)."""
+    """MPC.control (mpc.py:127-187) for `batch` robots, every step on the device: pre_process -> obstacle conversion
+    -> ADMM solve -> arrive rule.  Keyword set of the reference's MPC where it applies.
+
+    Without `robot_path`, every robot follows the one reference path `ref_path`.  With `robot_path` [B], `ref_path`
+    is a sequence of W paths and robot b follows path robot_path[b], as a batch of reference MPC objects that each own
+    their ref_path; a robot whose robot_path is outside [0, W) has no path (its reference holds its state and it is
+    reported as arrived).  With `enable_reverse` each waypoint carries a gear flag in its 4th row (+1 forward, -1
+    reverse; mpc.py:139-144): every path is cut into single-gear curves (split_path, mpc.py:232-249), the solver's
+    reference speed carries the gear's sign and a robot moves on to the next curve of its path when it reaches the end
+    of the current one (mpc.py:166-183).  cur_index is relative to the robot's curve, curve_index to its path."""
 
     def __init__(self, car_tuple, ref_path, batch, receding=10, sample_time=0.1, iter_num=4,
                  enable_reverse=False, obstacle_order=True, max_edge_num=5, max_obs_num=5,
-                 accelerated=True, goal_index_threshold=1, device=None, iter_threshold=0.2, **kwargs):
+                 accelerated=True, goal_index_threshold=1, device=None, iter_threshold=0.2, robot_path=None, **kwargs):
         self.lib = _cabi.load()
         self.enable_reverse = bool(enable_reverse)
         self.rda = RDA_solver(receding, car_tuple, max_edge_num, max_obs_num, iter_num=iter_num,
@@ -190,22 +240,42 @@ class BatchedMPC:
         self.dynamics, self.L = car_tuple.dynamics, float(car_tuple.wheelbase)
         self.obstacle_order = obstacle_order
         self.goal_index_threshold = goal_index_threshold
-        self.path = path_tensor(ref_path, self.device)
-        self.cur_index = torch.zeros(batch, dtype=torch.int32, device=self.device)
-        if self.enable_reverse:
-            # split_path (mpc.py:232-249): a new curve starts wherever the gear flag changes
-            flags = np.array([float(np.asarray(p, float).reshape(-1)[-1]) for p in ref_path])
-            cuts = [0] + [i for i in range(1, len(flags)) if flags[i] != flags[i - 1]] + [len(flags)]
-            self.curve_start = torch.as_tensor(cuts, dtype=torch.int32, device=self.device)
-            self.curve_gear = torch.as_tensor([flags[c] for c in cuts[:-1]], dtype=torch.float32, device=self.device)
-            self.n_curves = len(cuts) - 1
-            self.curve_index = torch.zeros(batch, dtype=torch.int32, device=self.device)
+        self.update_ref_path(ref_path, robot_path)
         init_vel = kwargs.get('init_vel')
         self.cur_vel = torch.zeros((batch, 2, receding), dtype=torch.float32, device=self.device)
         if init_vel is not None:
             self.cur_vel[:] = torch.as_tensor(init_vel, dtype=torch.float32, device=self.device)
         self.arrive = torch.zeros(batch, dtype=torch.int32, device=self.device)
         self._empty = None
+
+    def update_ref_path(self, ref_path, robot_path=None):
+        """MPC.update_ref_path (mpc.py:220-227) for the whole fleet: replace the path set (one path, or W paths with
+        robot_path [B] as in the constructor) and put every robot back at the start of its path's first curve.
+        cur_vel is kept, as in the reference."""
+        dev = self.device
+        paths = [ref_path] if robot_path is None else list(ref_path)
+        packed = {k: torch.as_tensor(v, device=dev).contiguous()
+                  for k, v in pack_paths(paths, self.enable_reverse).items()}
+        self.path, self.curve_start = packed['path'], packed['curve_start']
+        self.path_curve, self.curve_gear = packed['path_curve'], packed['curve_gear']
+        self.n_paths, self.n_curves = len(paths), packed['curve_gear'].shape[0]
+        if robot_path is None:
+            self.robot_path = torch.zeros(self.batch, dtype=torch.int32, device=dev)
+        else:
+            self.robot_path = torch.as_tensor(robot_path, dtype=torch.int32, device=dev).reshape(self.batch).contiguous()
+        self.cur_index = torch.zeros(self.batch, dtype=torch.int32, device=dev)
+        self.curve_index = torch.zeros(self.batch, dtype=torch.int32, device=dev)
+
+    def set_robot_path(self, robot_path, robots):
+        """Put the robots of the bool mask robots [B] on paths of the current set, robot_path [B] or one index for all
+        of them, at the start of the path's first curve: MPC.update_ref_path on those robots' MPCs.  On the device,
+        without a host synchronisation; an index outside [0, W) leaves the robot without a path."""
+        dev = self.device
+        robots = torch.as_tensor(robots, dtype=torch.bool, device=dev).reshape(self.batch)
+        robot_path = torch.as_tensor(robot_path, dtype=torch.int32, device=dev)
+        self.robot_path = torch.where(robots, robot_path, self.robot_path).contiguous()
+        self.cur_index = self.cur_index.masked_fill(robots, 0)
+        self.curve_index = self.curve_index.masked_fill(robots, 0)
 
     def _no_obstacles(self):
         if self._empty is None:
@@ -221,7 +291,7 @@ class BatchedMPC:
         pack_shapes / shapes_to_device (None: free space).  Instead of shapes, world: dict from
         pack_worlds / shapes_to_device, obstacle maps shared by the robots, with robot_world [B] the map of
         each robot (may be omitted with a single map).  Returns (u0 [B,2], info) where info holds
-        the solver's batched outputs plus 'arrive', 'nom_s', 'ref_s', 'cur_index'.  No host sync."""
+        the solver's batched outputs plus 'arrive', 'nom_s', 'ref_s', 'cur_index', 'curve_index'.  No host sync."""
         dev, B, T = self.device, self.batch, self.T
         if world is not None:
             if shapes is not None:
@@ -235,21 +305,16 @@ class BatchedMPC:
             ref_speed = torch.full((B,), float(ref_speed), dtype=torch.float32, device=dev) if np.isscalar(ref_speed) \
                 else torch.as_tensor(ref_speed, dtype=torch.float32, device=dev)
         ref_speed = ref_speed.to(dtype=torch.float32).contiguous()
-        solver_speed = ref_speed
-        if self.enable_reverse:
-            nom_s = torch.empty((B, 3, T + 1), dtype=torch.float32, device=dev)
-            ref_s = torch.empty((B, 3, T + 1), dtype=torch.float32, device=dev)
-            near = torch.empty(B, dtype=torch.int32, device=dev)
-            with torch.cuda.device(dev):
-                _cabi.check(self.lib.rda_pre_process_curves(
-                    B, T, _cabi.DYNAMICS[self.dynamics], self.dt, self.L, _ptr(state), _ptr(self.cur_vel), _ptr(ref_speed),
-                    _ptr(self.path), self.n_curves, _ptr(self.curve_start), _ptr(self.curve_index), _ptr(self.cur_index),
-                    0.1, 10, _ptr(nom_s), _ptr(ref_s), _ptr(near), _stream(dev)), 'rda_pre_process_curves')
-            gear = self.curve_gear[self.curve_index.long().clamp(max=self.n_curves - 1)]
-            solver_speed = (ref_speed * gear).contiguous()                      # gear_flag * ref_speed (mpc.py:161)
-        else:
-            nom_s, ref_s, near = pre_process_batch(state, self.cur_vel, ref_speed, self.path, self.cur_index,
-                                                   self.dynamics, self.dt, self.L, T)
+        nom_s = torch.empty((B, 3, T + 1), dtype=torch.float32, device=dev)
+        ref_s = torch.empty((B, 3, T + 1), dtype=torch.float32, device=dev)
+        near = torch.empty(B, dtype=torch.int32, device=dev)
+        solver_speed = torch.empty(B, dtype=torch.float32, device=dev)          # gear_flag * ref_speed (mpc.py:161)
+        with torch.cuda.device(dev):
+            _cabi.check(self.lib.rda_pre_process_paths(
+                B, T, _cabi.DYNAMICS[self.dynamics], self.dt, self.L, _ptr(state), _ptr(self.cur_vel), _ptr(ref_speed),
+                _ptr(self.path), self.n_paths, _ptr(self.path_curve), _ptr(self.curve_start), _ptr(self.curve_gear),
+                _ptr(self.robot_path), _ptr(self.curve_index), _ptr(self.cur_index), 0.1, 10, _ptr(nom_s), _ptr(ref_s),
+                _ptr(near), _ptr(solver_speed), _stream(dev)), 'rda_pre_process_paths')
         self.cur_index = near
         if (shapes is None and world is None) or self.N == 0:
             A, b, kind, count = self._no_obstacles()
@@ -262,18 +327,12 @@ class BatchedMPC:
                                                         self.obstacle_order)
         out = self.rda.iterative_solve_batch(nom_s, self.cur_vel, ref_s, solver_speed, A, b, kind, count, time_varying)
         with torch.cuda.device(dev):
-            if self.enable_reverse:
-                _cabi.check(self.lib.rda_post_process_gear(B, T, self.n_curves, _ptr(self.curve_start), self.goal_index_threshold,
-                                                           _ptr(near), _ptr(self.curve_index), _ptr(out['u']), _ptr(self.cur_vel),
-                                                           _ptr(self.arrive), _stream(dev)), 'rda_post_process_gear')
-            else:
-                _cabi.check(self.lib.rda_post_process(B, T, self.path.shape[0], self.goal_index_threshold, _ptr(near),
-                                                      _ptr(out['u']), _ptr(self.cur_vel), _ptr(self.arrive), _stream(dev)),
-                            'rda_post_process')
+            _cabi.check(self.lib.rda_post_process_paths(B, T, self.n_paths, _ptr(self.path_curve), _ptr(self.curve_start),
+                                                        _ptr(self.robot_path), self.goal_index_threshold, _ptr(near),
+                                                        _ptr(self.curve_index), _ptr(out['u']), _ptr(self.cur_vel),
+                                                        _ptr(self.arrive), _stream(dev)), 'rda_post_process_paths')
         info = dict(out)
-        info.update(arrive=self.arrive, nom_s=nom_s, ref_s=ref_s, cur_index=near)
-        if self.enable_reverse:
-            info['curve_index'] = self.curve_index
+        info.update(arrive=self.arrive, nom_s=nom_s, ref_s=ref_s, cur_index=near, curve_index=self.curve_index)
         return out['u'][:, :, 0], info
 
     def advance(self, state):
@@ -288,5 +347,4 @@ class BatchedMPC:
         self.rda.reset()
         self.cur_index.zero_()
         self.cur_vel.zero_()
-        if self.enable_reverse:
-            self.curve_index.zero_()
+        self.curve_index.zero_()
