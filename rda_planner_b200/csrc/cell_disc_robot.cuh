@@ -18,12 +18,6 @@
 extern "C" void rda_soc_stat(int newton);      // host statistics build only
 extern "C" void rda_dr_stat(int what);         // which cells reach the barrier programmes: 0 disjoint, 1 overlapping, +2 tilted
 #endif
-#ifndef RDA_DR_OVERLAP_FORMS
-#define RDA_DR_OVERLAP_FORMS 1                 // closed forms of the disc body overlapping a polygon (cases ii-v)
-#endif
-#ifndef RDA_DR_POINT_CONTACT
-#define RDA_DR_POINT_CONTACT 1                 // float64 closed forms of the disc body's point contacts (disc_point_contact)
-#endif
 
 namespace rda {
 
@@ -86,18 +80,10 @@ RDA_HD double soc_cone_grad(const SocQP<NV, MC>& P, int k, int r, double u, doub
 }
 
 // Feasible-start path following: damped Newton with backtracking on t*f0 + barrier, t = 1, MU, MU^2, ... up to TMAX
-// (duality gap (m + 2 nc)/t ~ 3e-11 at the end); intermediate centres only to a Newton decrement of RDA_SOC_CENTER (the
-// path is followed, not traced), the last one to 1e-9.  x must hold a strictly feasible point.  Measured on the committed
-// disc-body cases (CPU): MU 8 / centre 1e-9 -> 85 Newton steps per solve, MU 50 / 1e-2 -> 53, identical results.
-#ifndef RDA_SOC_MU
-#define RDA_SOC_MU 50.0
-#endif
-#ifndef RDA_SOC_TMAX
-#define RDA_SOC_TMAX 5.0e11
-#endif
-#ifndef RDA_SOC_CENTER
-#define RDA_SOC_CENTER 1e-2
-#endif
+// (duality gap (m + 2 nc)/t ~ 3e-11 at the end); intermediate centres only to a Newton decrement of BARRIER_CENTER (the
+// path is followed, not traced), the last one to 1e-9 — the path of coop_barrier (coop_ipm.cuh).  x must hold a strictly
+// feasible point.  Measured on the committed disc-body cases (CPU): MU 8 / centre 1e-9 -> 85 Newton steps per solve,
+// MU 50 / 1e-2 -> 53, identical results.
 template <int NV, int MC, typename Ctx>
 RDA_HD bool soc_barrier(SocQP<NV, MC>& P, Ctx& ctx) {
   const int lane = ctx.lane(), nl = ctx.nlanes();
@@ -105,7 +91,7 @@ RDA_HD bool soc_barrier(SocQP<NV, MC>& P, Ctx& ctx) {
   double t = 1.0;
   int newton = 0;
   for (int outer = 0; outer < 64; ++outer) {
-    const bool last = t >= RDA_SOC_TMAX;
+    const bool last = t >= BARRIER_TMAX;
     for (int itn = 0; itn < 30; ++itn) {
       ++newton;
       for (int i = lane; i < m; i += nl) {
@@ -157,7 +143,7 @@ RDA_HD bool soc_barrier(SocQP<NV, MC>& P, Ctx& ctx) {
       for (int k = lane; k < NV; k += nl) lam2 -= P.gr[k] * P.dx[k];
       lam2 = ctx.sum(lam2);
       if (!(lam2 == lam2)) return false;
-      if (lam2 < (last ? 1e-9 : RDA_SOC_CENTER)) break;
+      if (lam2 < (last ? 1e-9 : BARRIER_CENTER)) break;
       const double f0 = soc_value<NV, MC, Ctx>(P, P.x, t, ctx);
       double step = 1.0;
       bool moved = false;
@@ -174,7 +160,7 @@ RDA_HD bool soc_barrier(SocQP<NV, MC>& P, Ctx& ctx) {
       ctx.sync();
     }
     if (last) break;
-    t = rmin(t * RDA_SOC_MU, (double)RDA_SOC_TMAX);
+    t = rmin(t * BARRIER_MU, BARRIER_TMAX);
   }
   if (lane == 0) P.newton = newton;
 #if defined(RDA_SOC_STATS) && !defined(__CUDA_ARCH__)
@@ -412,7 +398,7 @@ RDA_HD void cell_front_dr(const RobotGeom& rb, int kind, int E, const float* A, 
       }
     }
   }
-  if (RDA_DR_POINT_CONTACT && searched_forms && !have && sep) {
+  if (searched_forms && !have && sep) {
     // POINT contacts (float64, disc_point_contact): each obstacle vertex whose normal cone can hold the contact direction,
     // or the centre of a disc obstacle
     const double c_ = cphi, s_ = sphi;
@@ -452,7 +438,7 @@ RDA_HD void cell_front_dr(const RobotGeom& rb, int kind, int E, const float* A, 
       }
     }
   }
-  if (RDA_DR_OVERLAP_FORMS && searched_forms && !have && !sep) {
+  if (searched_forms && !have && !sep) {
     // OVERLAPPING sets: the contact distance is zero, the numerator of the weighted margin is k0 - xi.y and the optimum sits
     // (ii) at a body point whose image lies strictly inside the obstacle (v = 0), (iii) on an obstacle edge strictly inside the
     // body (g = 0), (iv) at an obstacle vertex strictly inside the body, or (v) where the body's rim crosses an obstacle edge —
@@ -586,16 +572,6 @@ RDA_HD void cell_slow_dr(const RobotGeom& rb, CellWork<Real>& w, DiscSlowStore& 
   const double rr = rb.rad, bcx = rb.cx, bcy = rb.cy;
 #if defined(RDA_SOC_STATS) && !defined(__CUDA_ARCH__)
   rda_dr_stat((w.sep ? 0 : 1) + (w.xi_zero ? 0 : 2));
-#ifdef RDA_DR_DUMP
-  if (w.sep && !w.xi_zero) {
-    static int dumped = 0;
-    if (dumped < 12) { ++dumped;
-      fprintf(stderr, "DRCELL kind %d ne %d k0 %.9g cphi %.9g sphi %.9g xi %.9g %.9g ro2 %g r %g c %g %g best %.9g", w.g.kind, w.g.ne, (double)w.k0, (double)w.cphi, (double)w.sphi, (double)w.xi0, (double)w.xi1, (double)w.ro2, (double)rb.rad, (double)rb.cx, (double)rb.cy, (double)w.best);
-      for (int i = 0; i < w.g.ne; ++i) fprintf(stderr, " V %.9g %.9g", (double)w.g.vx[i], (double)w.g.vy[i]);
-      if (w.g.kind == 1) fprintf(stderr, " disc %.9g %.9g %.9g", (double)w.g.cx, (double)w.g.cy, (double)w.g.rad);
-      fprintf(stderr, "\n"); }
-  }
-#endif
 #endif
   if (lane == 0) {
     const CellGeom<Real>& g = w.g;

@@ -24,24 +24,11 @@ extern "C" void rda_case_stat(int line);
 #define RDA_CASE_STAT(line) ((void)0)
 #endif
 #include "rda_hd.h"
-// Acceptance of float32 closed-form candidates whose stationarity residual is limited by the resolution of float32
-// (edge-contact roots bracketed to one ulp of the edge parameter: residual up to 1e-4; edge x edge contacts: up to 1e-3).
-// Accepting them keeps ~90 % of the last pass' cells out of the float64 interior point iteration but costs parity:
-// tests/test_gpu_parity50.py at iteration 8: max state gap 7.9e-3 with, < 1e-3 without.  Off since the interior point
-// pass became warp-cooperative (cheap).
-#ifndef RDA_CELL_ACCEPT_CONV
-#define RDA_CELL_ACCEPT_CONV 0
-#endif
-#ifndef RDA_CELL_POLISH
-#define RDA_CELL_POLISH 0      // float64 polish of float32 edge-contact roots in the last pass (edge_contact_polish): halves the
-                               // interior point cells but measured SLOWER (all cell passes: the
-                               // kernel needs 168 registers with it, or spills when capped), so off
-#endif
-#ifndef RDA_CELL_EE_TANG
-#define RDA_CELL_EE_TANG 1e-4
-#endif
 
 namespace rda {
+
+// tangential residual of g accepted at the closed-form stationary point of a robot-edge x obstacle-edge contact (rounding only)
+constexpr double CELL_EE_TANG = 1e-4;
 
 enum { CELL_FAST_INACTIVE = 0, CELL_FAST_VERTEX = 1, CELL_SLOW_A = 2, CELL_SLOW_B = 3,
        CELL_OVERLAP_FREE = 4, CELL_FAILED = 5, CELL_NEEDS_SLOW = 6 };
@@ -141,47 +128,6 @@ struct CellWork {
   bool exact_zero_q, have;
   int path;
 };
-
-// ---- float64 polish of a robot-edge contact root (last pass only) ---------------------------------------------------
-// cell_front brackets the stationary point of the (weighted) margin along a body edge in the cell's own precision.  In
-// float32 that resolves the edge parameter to one ulp, which leaves a stationarity residual of up to 1e-4 when the
-// contact is close (the contact direction turns by |f|/distance per unit s) — more than the KKT acceptance allows, so
-// such cells used to go to the interior point iteration.  The last pass instead repeats the root search in float64 on
-// the float bracket (widened by a few ulps) and checks the KKT conditions in float64: same closed form, no loss of
-// parity.  Returns false when the bracket does not hold in float64 (the cell then goes to the interior point pass).
-struct EdgeRootD { double s, vx, vy, yx, yy, Nv, W2; };
-RDA_HD_NOINLINE bool edge_contact_polish(bool weighted, double lo, double hi, double yjx, double yjy, double fx, double fy,
-                                         double cphi, double sphi, double ox, double oy, double rad, double xi0, double xi1,
-                                         double k0, double ro2, EdgeRootD& r) {
-  const double wfx = cphi * fx - sphi * fy, wfy = sphi * fx + cphi * fy, xf = xi0 * fx + xi1 * fy;
-  double hv = 0;
-  auto eval = [&](double sc) {
-    r.s = sc;
-    r.yx = yjx + sc * fx; r.yy = yjy + sc * fy;
-    const double rx = (cphi * r.yx - sphi * r.yy) - ox, ry = (sphi * r.yx + cphi * r.yy) - oy;
-    const double rn = sqrt(rx * rx + ry * ry);
-    r.vx = rx / rn; r.vy = ry / rn;
-    r.Nv = k0 - (xi0 * r.yx + xi1 * r.yy) - (rn - rad);
-    const double Np = -xf - (r.vx * wfx + r.vy * wfy);
-    r.W2 = weighted ? 1.0 + (r.yx * r.yx + r.yy * r.yy) / ro2 : 1.0;
-    hv = weighted ? Np * r.W2 - r.Nv * (r.yx * fx + r.yy * fy) / ro2 : Np;
-  };
-  const double pad = 1e-6;
-  lo = rmax(lo - pad, 0.0); hi = rmin(hi + pad, 1.0);
-  eval(lo); double flo = hv; if (!(flo > 0) || (weighted && !(r.Nv > 0))) return false;
-  eval(hi); double fhi = hv; if (!(fhi < 0) || (weighted && !(r.Nv > 0))) return false;
-  int side = 0;
-  for (int itn = 0; itn < 60; ++itn) {
-    const double w = hi - lo;
-    double sc = lo + w * (flo / (flo - fhi));
-    sc = rclamp(sc, lo + 0.02 * w, hi - 0.02 * w);
-    eval(sc);
-    if (hv > 0) { lo = sc; flo = hv; if (side > 0) fhi *= 0.5; side = 1; }
-    else { hi = sc; fhi = hv; if (side < 0) flo *= 0.5; side = -1; }
-    if (hi - lo < 1e-14 || hv == 0) break;
-  }
-  return !weighted || r.Nv > 0;
-}
 
 // ---- stage 1: geometry relative to the robot reference point and the closed-form cases ----------
 // LEAN = true stops after the two cases that need no search (xi = 0 and a non-negative margin): the
@@ -412,8 +358,6 @@ RDA_HD void cell_front(const RobotGeom& rb, int kind, int E, const float* A, con
       // h at the bracket ends (flo > 0 at lo, fhi < 0 at hi) where it was evaluated inside the region N > 0
       Real flo = 0, fhi = 0;
       bool vlo = false, vhi = false;
-      bool conv = false;             // the root is bracketed by valid end values to the resolution of s
-      bool convf = false;            // ... whether or not such a root is accepted as it is (RDA_CELL_ACCEPT_CONV)
       if (!weighted) {
         eval((Real)0); const Real h0 = hv;
         eval((Real)1); const Real h1 = hv;
@@ -468,8 +412,6 @@ RDA_HD void cell_front(const RobotGeom& rb, int kind, int E, const float* A, con
           if (hi - lo < tol || abs_(sc - sprev) < tol || (valid && hv == (Real)0)) break;
           sprev = sc;
         }
-        conv = RDA_CELL_ACCEPT_CONV && vlo && vhi && hi - lo < (Real)4 * tol;
-        convf = vlo && vhi && hi - lo < (Real)4 * tol;
         if (!weighted) sA = sc;
       }
       if (!bracket) continue;
@@ -477,8 +419,8 @@ RDA_HD void cell_front(const RobotGeom& rb, int kind, int E, const float* A, con
       const Real rvx = cphi * vx_ + sphi * vy_, rvy = -sphi * vx_ + cphi * vy_;   // R'v
       const Real tolc = sizeof(Real) == 4 ? (Real)1e-5 : (Real)1e-11;
       // tangential residual of g on the edge: h is the tangential component of the gradient scaled by W^2 |f| (steep: a
-      // slope of 1e4..1e5 per unit s with the metric's ro), so ONE float32 ulp of s leaves a residual of 1e-4; a root
-      // bracketed by valid end values to that resolution (conv) is accepted as it is
+      // slope of 1e4..1e5 per unit s with the metric's ro), so ONE float32 ulp of s leaves a residual of 1e-4; such a root
+      // fails this test and its cell goes on to the interior point iteration (DESIGN.md §3.1)
       const Real tole = sizeof(Real) == 4 ? (Real)3e-5 : (Real)1e-9;
       bool cone_ok = true;
       if (kind != RDA_OBS_CIRCLE) {
@@ -494,7 +436,7 @@ RDA_HD void cell_front(const RobotGeom& rb, int kind, int E, const float* A, con
           const Real cgx = -rvx - xi0, cgy = -rvy - xi1;
           // g must be a non-negative multiple of the edge normal: no tangential component left
           const Real tang = abs_(cgx * fx + cgy * fy) * rsqrt_(fx * fx + fy * fy);
-          if (cgx * (Real)rb.nx[j] + cgy * (Real)rb.ny[j] >= -tolc && (tang <= tole || conv)) {
+          if (cgx * (Real)rb.nx[j] + cgy * (Real)rb.ny[j] >= -tolc && tang <= tole) {
             v0 = vx_; v1 = vy_; g0 = cgx; g1 = cgy;
             exact_zero_q = true; have = true; RDA_CASE_STAT(__LINE__); path = CELL_FAST_VERTEX;
           }
@@ -503,34 +445,9 @@ RDA_HD void cell_front(const RobotGeom& rb, int kind, int E, const float* A, con
         const Real tau = Nv / W2;
         const Real cgx = -tau * yx / ro2 - rvx - xi0, cgy = -tau * yy / ro2 - rvy - xi1;
         const Real tang = abs_(cgx * fx + cgy * fy) * rsqrt_(fx * fx + fy * fy);
-        if (cgx * (Real)rb.nx[j] + cgy * (Real)rb.ny[j] >= -tolc && (tang <= tole || conv)) {
+        if (cgx * (Real)rb.nx[j] + cgy * (Real)rb.ny[j] >= -tolc && tang <= tole) {
           v0 = vx_; v1 = vy_; g0 = cgx; g1 = cgy;
           have = true; RDA_CASE_STAT(__LINE__); path = CELL_FAST_VERTEX;
-        }
-      }
-      if (RDA_CELL_POLISH && EXTRA && sizeof(Real) == 4 && !have && convf) {
-        // float32 resolved the root to one ulp of s but not the KKT residual: polish in float64 (edge_contact_polish)
-        EdgeRootD rt;
-        if (edge_contact_polish(weighted, (double)lo, (double)hi, (double)yjx, (double)yjy, (double)fx, (double)fy, (double)cphi,
-                                (double)sphi, (double)ox, (double)oy, (double)rad, (double)xi0, (double)xi1, (double)k0, (double)ro2, rt)) {
-          const double c_ = cphi, s_ = sphi;
-          const double rvxd = c_ * rt.vx + s_ * rt.vy, rvyd = -s_ * rt.vx + c_ * rt.vy;
-          bool okd = true;
-          if (kind != RDA_OBS_CIRCLE) {
-            const int ip = (ce_i + ne - 1) % ne, inx = (ce_i + 1) % ne;
-            const double epx = (double)g.vx[ce_i] - (double)g.vx[ip], epy = (double)g.vy[ce_i] - (double)g.vy[ip];
-            const double enx = (double)g.vx[inx] - (double)g.vx[ce_i], eny = (double)g.vy[inx] - (double)g.vy[ce_i];
-            okd = (rt.vx * epx + rt.vy * epy >= -1e-9 * sqrt(epx * epx + epy * epy)) &&
-                  (rt.vx * enx + rt.vy * eny <= 1e-9 * sqrt(enx * enx + eny * eny));
-          }
-          const double tau = weighted ? rt.Nv / rt.W2 : 0.0;
-          const double cgx = -tau * rt.yx / (double)ro2 - rvxd - (double)xi0, cgy = -tau * rt.yy / (double)ro2 - rvyd - (double)xi1;
-          const double tang = fabs(cgx * (double)fx + cgy * (double)fy) / sqrt((double)fx * fx + (double)fy * fy);
-          okd = okd && (weighted ? rt.Nv > 0 : rt.Nv <= 0) && cgx * (double)rb.nx[j] + cgy * (double)rb.ny[j] >= -1e-9 && tang <= 1e-7;
-          if (okd) {
-            v0 = (Real)rt.vx; v1 = (Real)rt.vy; g0 = (Real)cgx; g1 = (Real)cgy;
-            exact_zero_q = !weighted; have = true; RDA_CASE_STAT(__LINE__); path = CELL_FAST_VERTEX;
-          }
         }
       }
     }
@@ -573,7 +490,7 @@ RDA_HD void cell_front(const RobotGeom& rb, int kind, int E, const float* A, con
         const Real cgx = -tau * yx / ro2 - rvx - xi0, cgy = -tau * yy / ro2 - rvy - xi1;
         // s* is a stationary point in closed form: the tangential component of g is rounding only (bounded loosely)
         const Real tang = abs_(cgx * fx + cgy * fy) * rsqrt_(fx * fx + fy * fy);
-        if (!(cgx * (Real)rb.nx[j] + cgy * (Real)rb.ny[j] >= -tolc && tang <= (Real)RDA_CELL_EE_TANG)) continue;
+        if (!(cgx * (Real)rb.nx[j] + cgy * (Real)rb.ny[j] >= -tolc && tang <= (Real)CELL_EE_TANG)) continue;
         v0 = nix; v1 = niy; g0 = cgx; g1 = cgy;
         have = true; RDA_CASE_STAT(__LINE__); path = CELL_FAST_VERTEX;
       }

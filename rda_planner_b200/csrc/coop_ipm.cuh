@@ -261,26 +261,19 @@ RDA_HD double coop_barrier_value(const CoopQP<NV, MC>& P, const double* x, doubl
   return ctx.max((double)bad) > 0 ? 1e300 : f;
 }
 
+// The barrier path t = 1, BARRIER_MU, BARRIER_MU^2, ... BARRIER_TMAX is followed, not traced: intermediate centres only to a
+// Newton decrement of BARRIER_CENTER, the last one to 1e-9 (r02: MU 8 with every centre to 1e-9 needed 85 Newton steps per
+// solve, MU 50 with 1e-2 needs 53, same results to the last digit of the float32 outputs).
+constexpr double BARRIER_MU = 50.0, BARRIER_TMAX = 5.0e11, BARRIER_CENTER = 1e-2;
+
 template <int NV, int MC, typename Ctx>
 RDA_HD bool coop_barrier(CoopQP<NV, MC>& P, Ctx& ctx) {
   const int lane = ctx.lane(), nl = ctx.nlanes();
   const int m = P.m, tv = P.tv;
-  // The path t = 1, MU, MU^2, ... TMAX is followed, not traced: intermediate centres only to a Newton decrement of
-  // RDA_BARRIER_CENTER, the last one to 1e-9 (r02: MU 8 with every centre to 1e-9 needed 85 Newton steps per solve, MU 50
-  // with 1e-2 needs 53, same results to the last digit of the float32 outputs).
-#ifndef RDA_BARRIER_MU
-#define RDA_BARRIER_MU 50.0
-#endif
-#ifndef RDA_BARRIER_TMAX
-#define RDA_BARRIER_TMAX 5.0e11
-#endif
-#ifndef RDA_BARRIER_CENTER
-#define RDA_BARRIER_CENTER 1e-2
-#endif
   double t = 1.0;
   int newton = 0;
   for (int outer = 0; outer < 64; ++outer) {
-    const bool last = t >= RDA_BARRIER_TMAX;
+    const bool last = t >= BARRIER_TMAX;
     for (int it = 0; it < 30; ++it) {
       ++newton;
       // slack reciprocals
@@ -328,7 +321,7 @@ RDA_HD bool coop_barrier(CoopQP<NV, MC>& P, Ctx& ctx) {
       for (int k = lane; k < NV; k += nl) lam2 -= P.rd[k] * P.ra[k];
       lam2 = ctx.sum(lam2);
       if (!(lam2 == lam2)) return false;
-      if (lam2 < (last ? 1e-9 : RDA_BARRIER_CENTER)) break;
+      if (lam2 < (last ? 1e-9 : BARRIER_CENTER)) break;
       const double f0 = coop_barrier_value<NV, MC, Ctx>(P, P.x, t, ctx);
       double step = 1.0;
       bool moved = false;
@@ -345,7 +338,7 @@ RDA_HD bool coop_barrier(CoopQP<NV, MC>& P, Ctx& ctx) {
       ctx.sync();
     }
     if (last) break;
-    t = rmin(t * RDA_BARRIER_MU, (double)RDA_BARRIER_TMAX);
+    t = rmin(t * BARRIER_MU, BARRIER_TMAX);
   }
   RDA_STAT(2, newton);
   (void)newton;

@@ -2,8 +2,8 @@
 //
 // One ADMM iteration (rda_solver.py:612-637) is five launches on the caller's stream:
 //   k_su      one warp per planning instance: su-QP (su_solver.cuh), state staged in shared memory
-//   k_cells_fast / k_cells_mid / k_cells_slow   one thread per (instance, obstacle, stage) cell: (lam, mu, z) +
-//             xi/zeta update + residual partial sums + the next su-QP's hinge inputs (cell_solver.cuh)
+//   k_cells_fast / k_cells_mid   one thread per (instance, obstacle, stage) cell, k_cells_slow_coop one warp per cell:
+//             (lam, mu, z) + xi/zeta update + residual partial sums + the next su-QP's hinge inputs (cell_solver.cuh)
 //   k_finalize per instance: residuals, early-stop flag (:594-596)
 // No host synchronisation, no allocation, CUDA-graph capturable.
 #include <cuda_runtime.h>
@@ -58,16 +58,10 @@ struct rda_handle {
   // persistent single-launch ADMM for small batches (k_admm_small, SURVEY §8 f4)
   int small_mode;        // -1: batches up to small_max instances, 0: never, 1: always when the state fits (RDA_B200_SMALL)
   int small_max, small_ok, small_bulk;
-  int small_coop;        // interior point cells of the persistent kernel one per warp (RDA_B200_SMALL_COOP, default 1)
   SmallLayout small_L;
   float su_prune;        // hinge pruning margin of the su-QP (su_solver.cuh; RDA_B200_SU_PRUNE, 0 = off)
-  int slow_cpw, slow_ctas;   // k_cells_slow: cells per warp, CTAs per SM (RDA_B200_SLOW_CPW / RDA_B200_SLOW_CTAS)
-  int slow_coop;             // warp-cooperative last pass, one cell per warp (RDA_B200_SLOW_COOP, default 1)
-  int mid_ctas;              // k_cells_mid CTAs per SM (RDA_B200_MID_CTAS)
   int extra_min;             // sub-batches of at least this many instances run k_cells_extra before the cooperative pass (RDA_B200_EXTRA_MIN)
-  int dr_coop;               // disc body: barrier cells one per warp (RDA_B200_DR_COOP, default 1)
-  int slow_adapt;            // fewer cells per warp when the list fits one wave (RDA_B200_SLOW_ADAPT, default 0: measured slower)
-  int split_min;         // smallest batch that is split (RDA_B200_SPLIT_MIN, default 2048)
+  int split_min;        // smallest batch that is split (RDA_B200_SPLIT_MIN, default 2048)
   int parts;             // number of sub-batches, 1..4 (RDA_B200_SPLIT_PARTS, default 2)
 };
 
@@ -542,12 +536,7 @@ __device__ __forceinline__ void rows_preload(const DevPtrs& d, const CellIn& c, 
 
 // Second pass: the searched closed forms (vertex / edge contact, overlap cases) for the cells of the
 // first worklist, one thread per entry; what is still unresolved goes to the second worklist.
-#ifdef RDA_MID_MINBLOCKS
-#define RDA_MID_BOUNDS __launch_bounds__(128, RDA_MID_MINBLOCKS)
-#else
-#define RDA_MID_BOUNDS __launch_bounds__(128)
-#endif
-__global__ void RDA_MID_BOUNDS k_cells_mid(DevPtrs d, RobotGeom rb, float ro2, float theta) {
+__global__ void __launch_bounds__(128) k_cells_mid(DevPtrs d, RobotGeom rb, float ro2, float theta) {
   const int count = d.wl_count[0];
   const int lane = threadIdx.x & 31;
   for (int base = blockIdx.x * blockDim.x; base < count; base += gridDim.x * blockDim.x) {
@@ -555,11 +544,9 @@ __global__ void RDA_MID_BOUNDS k_cells_mid(DevPtrs d, RobotGeom rb, float ro2, f
     const bool live = wi < count;
     bool need = false;
     long long idx = 0;
-    int kind_of = RDA_OBS_POLYGON;
     if (live) {
       idx = d.worklist[wi];
       CellIn c = cell_load(d, idx);
-      kind_of = c.kind;
       RowsLocal rows;
       rows_preload(d, c, rows);
       CellWork<float> w;
@@ -578,8 +565,7 @@ __global__ void RDA_MID_BOUNDS k_cells_mid(DevPtrs d, RobotGeom rb, float ro2, f
     unsigned m = __ballot_sync(0xffffffffu, need);
     if (m) {
       int leader = __ffs(m) - 1, pos = 0;
-      const unsigned mc = __ballot_sync(m, need && kind_of == RDA_OBS_CIRCLE);
-      if (lane == leader) { pos = atomicAdd(&d.wl_count[1], __popc(m)); if (mc) atomicAdd(&d.wl_count[3], __popc(mc)); }
+      if (lane == leader) pos = atomicAdd(&d.wl_count[1], __popc(m));
       pos = __shfl_sync(0xffffffffu, pos, leader);
       if (need) d.worklist2[pos + __popc(m & ((1u << lane) - 1))] = (int)idx;
     }
@@ -588,59 +574,12 @@ __global__ void RDA_MID_BOUNDS k_cells_mid(DevPtrs d, RobotGeom rb, float ro2, f
   }
 }
 
-// One thread per worklist entry, RDA_SLOW_CPW entries per warp.  The pass is a latency tail (a few thousand
-// cells, each a serial interior point iteration with its own iteration count and fallbacks): fewer cells
-// per warp means less divergence to serialise and more warps to hide latency; the idle lanes cost nothing
-// because the SMs are otherwise empty.
-#ifndef RDA_SLOW_MINBLOCKS
-#define RDA_SLOW_MINBLOCKS 16
-#endif
-#ifndef RDA_SLOW_CPW
-#define RDA_SLOW_CPW 32
-#endif
-__global__ void __launch_bounds__(64, RDA_SLOW_MINBLOCKS) k_cells_slow(DevPtrs d, RobotGeom rb, float ro2, float theta, int cpw, int adapt) {
-  const int count = d.wl_count[1];
-  const int lane = threadIdx.x & 31;
-  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int nwarps = (gridDim.x * blockDim.x) >> 5;
-  // Disc cells run the (long, strongly divergent) barrier iteration: when the list is mostly discs and short enough, one
-  // cell per warp (r02: 6.5x on BASELINE config C at 128 instances); polygon lists are fastest packed 32 per warp.
-  if (2 * d.wl_count[3] > count && count <= nwarps) cpw = 1;
-  // optional: as few cells per warp as one wave of the grid allows.  Measured slower at 16 384 instances — the pass is bound
-  // by issue slots and local-memory transactions, which full warps use far better.
-  if (adapt) cpw = min(cpw, max(1, (count + nwarps - 1) / nwarps));
-  if (lane >= cpw) return;
-  for (int wi = warp * cpw + lane; wi < count; wi += nwarps * cpw) {
-    const long long idx = d.worklist2[wi];
-    CellIn c = cell_load(d, idx);
-    CellWork<float> w;
-    cell_front<float, false, true>(rb, c.kind, d.E, c.A, c.bb, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0, c.xi1, ro2, w);
-    if (!w.have) {
-      CellSlowStore S;
-      SeqCtx ctx;
-      cell_slow<float, SeqCtx>(rb, w, S, ctx);
-    }
-    CellOut<float> out;
-    cell_back<float>(rb, w, c.zeta, theta, out);
-    float hm2 = 0.f, dual = 0.f;
-    if (out.path == CELL_FAILED) {
-      // "Update Lam Mu Fail": previous duals kept, residual inf (:791-793)
-      dual = INFINITY;
-      atomicOr(&d.status[c.b], RDA_ST_CELL_FALLBACK);
-    } else {
-      cell_store(d, c, out, &hm2, &dual);
-    }
-    atomicAdd(&d.resi_acc[2 * c.b], hm2);
-    atomicAdd(&d.resi_acc[2 * c.b + 1], dual);
-    atomicAdd(&d.counters[out.path == CELL_FAILED ? 2 : 1], 1);
-  }
-}
-
 // ------------------------------------------------------------------------------------------------
-// Disc body (car_tuple.cone_type 'norm2', rda_solver.py:1034-1039; cell_disc_robot.cuh).  Two passes over the
+// Disc body (car_tuple.cone_type 'norm2', rda_solver.py:1034-1039; cell_disc_robot.cuh).  Three passes over the
 // same worklist machinery: k_cells_dr solves every cell whose hinge is inactive in closed form (one thread per
-// cell, coalesced like the first polygon pass) and lists the rest; k_cells_dr_slow runs the two-cone barrier
-// programmes of the listed cells, one cell per thread.
+// cell, coalesced like the first polygon pass) and lists the rest; k_cells_dr_mid tries the searched closed forms
+// of the listed cells, one cell per thread; k_cells_dr_slow_coop runs the two-cone barrier programmes of what is
+// left, one cell per warp.
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(128) k_cells_dr(DevPtrs d, RobotGeom rb, float ro2, float theta) {
   const int NT = d.N * d.T;
@@ -677,40 +616,6 @@ __global__ void __launch_bounds__(128) k_cells_dr(DevPtrs d, RobotGeom rb, float
     }
     const unsigned solved = __ballot_sync(0xffffffffu, live && !need);
     if (lane == 0 && solved) atomicAdd(&d.counters[0], __popc(solved));
-  }
-}
-
-__global__ void __launch_bounds__(64) k_cells_dr_slow(DevPtrs d, RobotGeom rb, float ro2, float theta) {
-  const int count = d.wl_count[1];
-  const int lane = threadIdx.x & 31;
-  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int nwarps = (gridDim.x * blockDim.x) >> 5;
-  // the barrier iteration is long and its length differs from cell to cell: one cell per warp while the list is
-  // short enough to give every cell its own warp, packed otherwise
-  const int cpw = count <= nwarps ? 1 : 32;
-  if (lane >= cpw) return;
-  for (int wi = warp * cpw + lane; wi < count; wi += nwarps * cpw) {
-    const long long idx = d.worklist2[wi];
-    CellIn c = cell_load(d, idx);
-    CellWork<float> w;
-    cell_front_dr<float>(rb, c.kind, d.E, c.A, c.bb, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0, c.xi1, ro2, w);
-    if (!w.have) {
-      DiscSlowStore S;
-      SeqCtx ctx;
-      cell_slow_dr<float, SeqCtx>(rb, w, S, ctx);
-    }
-    CellOut<float> out;
-    cell_back_dr<float>(rb, w, c.zeta, theta, out);
-    float hm2 = 0.f, dual = 0.f;
-    if (out.path == CELL_FAILED) {
-      dual = INFINITY;                                   // "Update Lam Mu Fail": previous duals kept (:791-793)
-      atomicOr(&d.status[c.b], RDA_ST_CELL_FALLBACK);
-    } else {
-      cell_store(d, c, out, &hm2, &dual);
-    }
-    atomicAdd(&d.resi_acc[2 * c.b], hm2);
-    atomicAdd(&d.resi_acc[2 * c.b + 1], dual);
-    atomicAdd(&d.counters[out.path == CELL_FAILED ? 2 : 1], 1);
   }
 }
 
@@ -751,15 +656,17 @@ __global__ void __launch_bounds__(128) k_cells_dr_mid(DevPtrs d, RobotGeom rb, f
   }
 }
 
+// warps (cells) per CTA of the warp-cooperative passes k_cells_dr_slow_coop and k_cells_slow_coop
+constexpr int COOP_WARPS = 4;
+
 // one cell per WARP: the two-cone barrier iterations spread over the lanes, the problem in shared memory
-constexpr int DR_COOP_WARPS = 4;
-__global__ void __launch_bounds__(32 * DR_COOP_WARPS) k_cells_dr_slow_coop(DevPtrs d, RobotGeom rb, float ro2, float theta) {
-  __shared__ DiscSlowStore store[DR_COOP_WARPS];
+__global__ void __launch_bounds__(32 * COOP_WARPS) k_cells_dr_slow_coop(DevPtrs d, RobotGeom rb, float ro2, float theta) {
+  __shared__ DiscSlowStore store[COOP_WARPS];
   const int count = d.wl_count[4];          // what k_cells_dr_mid left, in d.worklist
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   DiscSlowStore& S = store[warp];
   WarpCtx ctx;
-  for (int wi = blockIdx.x * DR_COOP_WARPS + warp; wi < count; wi += gridDim.x * DR_COOP_WARPS) {
+  for (int wi = blockIdx.x * COOP_WARPS + warp; wi < count; wi += gridDim.x * COOP_WARPS) {
     const long long idx = d.worklist[wi];
     CellIn c;
     CellWork<float> w;
@@ -780,6 +687,7 @@ __global__ void __launch_bounds__(32 * DR_COOP_WARPS) k_cells_dr_slow_coop(DevPt
       cell_back_dr<float>(rb, w, c.zeta, theta, out);
       float hm2 = 0.f, dual = 0.f;
       if (out.path == CELL_FAILED) {
+        // "Update Lam Mu Fail": previous duals kept, residual inf (:791-793)
         dual = INFINITY;
         atomicOr(&d.status[c.b], RDA_ST_CELL_FALLBACK);
       } else {
@@ -834,14 +742,12 @@ __global__ void __launch_bounds__(128) k_cells_extra(DevPtrs d, RobotGeom rb, fl
   }
 }
 
-// Warp-cooperative variant of the last pass (RDA_B200_SLOW_COOP=1): ONE cell per warp, the interior point iteration of
-// coop_ipm.cuh spread over the lanes (rows, vector components and Newton-matrix entries), the problem in shared memory.
-// Round 1 measured it slower than one thread per cell — with 5 % of the cells in this pass; since the closed forms of
-// round 2 leave 0.1 % (~13 000 cells at 16 384 instances, three waves of warps) the pass is a pure latency tail, which is
-// what cooperation shortens.
-constexpr int SLOW_COOP_WARPS = 4;
-__global__ void __launch_bounds__(32 * SLOW_COOP_WARPS) k_cells_slow_coop(DevPtrs d, RobotGeom rb, float ro2, float theta, int from_extra) {
-  __shared__ CellSlowStore store[SLOW_COOP_WARPS];
+// Last pass, warp-cooperative: ONE cell per warp, the interior point iteration of coop_ipm.cuh spread over the lanes (rows,
+// vector components and Newton-matrix entries), the problem in shared memory.  Round 1 measured it slower than one thread per
+// cell — with 5 % of the cells in this pass; since the closed forms of round 2 leave 0.1 % (~13 000 cells at 16 384
+// instances, three waves of warps) the pass is a pure latency tail, which is what cooperation shortens (DESIGN.md §3.1).
+__global__ void __launch_bounds__(32 * COOP_WARPS) k_cells_slow_coop(DevPtrs d, RobotGeom rb, float ro2, float theta, int from_extra) {
+  __shared__ CellSlowStore store[COOP_WARPS];
   // from_extra: the list k_cells_extra left — d.worklist (the searched pass' list, consumed by now) with its own counter;
   // otherwise the searched pass' own leftovers (small batches: one launch less, lane 0 runs the EXTRA closed forms)
   const int count = from_extra ? d.wl_count[4] : d.wl_count[1];
@@ -849,7 +755,7 @@ __global__ void __launch_bounds__(32 * SLOW_COOP_WARPS) k_cells_slow_coop(DevPtr
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   CellSlowStore& S = store[warp];
   WarpCtx ctx;
-  for (int wi = blockIdx.x * SLOW_COOP_WARPS + warp; wi < count; wi += gridDim.x * SLOW_COOP_WARPS) {
+  for (int wi = blockIdx.x * COOP_WARPS + warp; wi < count; wi += gridDim.x * COOP_WARPS) {
     const long long idx = list[wi];
     CellIn c;
     CellWork<float> w;
@@ -918,9 +824,9 @@ __global__ void k_finalize(DevPtrs d, RobotGeom rb, float thr) {
 // ------------------------------------------------------------------------------------------------
 // SURVEY.md §8 f4: the whole ADMM loop of one (small) instance in ONE launch, one CTA per instance, every piece of
 // warm-start state staged in shared memory for the duration of the solve (HBM is touched once on the way in and
-// once on the way out).  Warp 0 runs the su-QP (same code as k_su), all warps the cells (first the lean closed
-// forms, then the searched ones and the interior point fall-back in the same thread), thread 0 the residual /
-// early-stop rule.  The kernel reuses the device functions of the streaming kernels through a DevPtrs whose
+// once on the way out).  Warp 0 runs the su-QP (same code as k_su), all threads the closed forms of the cells (one
+// cell per thread), all warps the interior point iteration of the cells those leave (one cell per warp, as
+// k_cells_slow_coop), thread 0 the residual / early-stop rule.  The kernel reuses the device functions of the streaming kernels through a DevPtrs whose
 // pointers address shared memory, so the arithmetic is identical; instances progress independently (no grid-wide
 // barrier between the ADMM phases).
 // ------------------------------------------------------------------------------------------------
@@ -932,7 +838,7 @@ static SmallLayout small_layout(int T, int N, int E, int R, size_t su_bytes) {
   L.lam = take(4 * N * E * T); L.mu = take(4 * N * R * T); L.z = take(4 * NT); L.xi = take(8 * NT); L.zeta = take(4 * NT);
   L.dis = take(4 * T); L.coef = take(20 * NT); L.pref = take(8 * T); L.cur_s = take(12 * (T + 1)); L.cur_u = take(8 * T);
   L.ref_s = take(12 * (T + 1)); L.misc = take(128); L.hs = take(16 * NT); L.su = take(su_bytes);
-  // cells left over by the closed forms (indices) and one interior point problem per warp (cooperative pass)
+  // which cells the closed forms left (one flag per cell) and one interior point problem per warp (cooperative pass)
   L.wl = take(4 * (NT + 1)); L.slow = take(4 * sizeof(CellSlowStore));
   L.total = (int)((o + 15) & ~(size_t)15);
   return L;
@@ -970,10 +876,12 @@ __device__ __forceinline__ void bulk_commit_wait() {
   asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
+// Two resident CTAs per SM (small_max, and the staged state in shared memory): the register budget that leaves lets ptxas
+// keep the su-QP's working set in registers (without the bound it settles at 168 and spills in the float64 build).
 template <typename Real>
-__global__ void __launch_bounds__(128) k_admm_small(DevPtrs d, SuParams P, RobotGeom rb, float ro2, float theta, float thr,
+__global__ void __launch_bounds__(128, 2) k_admm_small(DevPtrs d, SuParams P, RobotGeom rb, float ro2, float theta, float thr,
                                                     int iter_num, SmallLayout L, const float* nom_s, const float* nom_u,
-                                                    const float* ref_s, const float* ref_speed, rda_outputs out, int use_bulk, int coop) {
+                                                    const float* ref_s, const float* ref_speed, rda_outputs out, int use_bulk) {
   extern __shared__ __align__(16) char smem[];
   const int b = blockIdx.x;
   if (b >= d.B) return;
@@ -1034,41 +942,36 @@ __global__ void __launch_bounds__(128) k_admm_small(DevPtrs d, SuParams P, Robot
     }
     __syncthreads();
     if (has_obs) {
-      int* wl = (int*)(smem + L.wl);                 // wl[0]: number of listed cells, wl[1..]: their indices
-      if (tid == 0) wl[0] = 0;
-      __syncthreads();
+      // Residual terms are summed in a fixed order (per thread, then over the lanes, then warp by warp) so that a solve
+      // reproduces its residuals bit for bit.  wl[1 + idx]: whether cell idx is left to the interior point pass below.
+      int* wl = (int*)(smem + L.wl);
+      const int warp = tid >> 5, lane = tid & 31, nwarps = nth >> 5;
+      float hm2s = 0.f, duals = 0.f;
       for (int idx = tid; idx < NT; idx += nth) {
         CellIn c = cell_load(ds, idx);
         CellWork<float> w;
         cell_front<float, false, true>(rb, c.kind, E, c.A, c.bb, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0, c.xi1, ro2, w);
-        if (!w.have) {
-          if (coop) { wl[1 + atomicAdd(&wl[0], 1)] = idx; continue; }      // interior point pass below, one cell per warp
-          CellSlowStore S;
-          SeqCtx sc;
-          cell_slow<float, SeqCtx>(rb, w, S, sc);
-        }
+        wl[1 + idx] = !w.have;
+        if (!w.have) continue;
         CellOut<float> o;
         cell_back<float>(rb, w, c.zeta, theta, o);
         float hm2 = 0.f, dual = 0.f;
-        if (o.path == CELL_FAILED) {
-          dual = INFINITY;
-          atomicOr(&ds.status[0], RDA_ST_CELL_FALLBACK);
-        } else {
-          cell_store(ds, c, o, &hm2, &dual);
-        }
-        atomicAdd(&ds.resi_acc[0], hm2);
-        atomicAdd(&ds.resi_acc[1], dual);
-        atomicAdd(&d.counters[o.path == CELL_FAILED ? 2 : ((o.path == CELL_SLOW_A || o.path == CELL_SLOW_B) ? 1 : 0)], 1);
+        cell_store(ds, c, o, &hm2, &dual);
+        hm2s += hm2;
+        duals += dual;
+        atomicAdd(&d.counters[0], 1);
       }
-      if (coop) {
-        // the cells the closed forms left: one per warp, interior point iteration spread over the lanes (coop_ipm.cuh),
-        // the problem in shared memory — as k_cells_slow_coop of the streaming path
-        __syncthreads();
-        const int nlist = wl[0], warp = tid >> 5, lane = tid & 31;
-        CellSlowStore& S = ((CellSlowStore*)(smem + L.slow))[warp];
-        WarpCtx ctx;
-        for (int wi = warp; wi < nlist; wi += (nth >> 5)) {
-          const int idx = wl[1 + wi];
+      // the cells the closed forms left, in index order, the k-th to warp k % nwarps: interior point iteration spread over
+      // the lanes (coop_ipm.cuh), the problem in shared memory — as k_cells_slow_coop of the streaming path
+      __syncthreads();
+      CellSlowStore& S = ((CellSlowStore*)(smem + L.slow))[warp];
+      WarpCtx ctx;
+      int rank = 0;
+      for (int base = 0; base < NT; base += 32) {
+        unsigned m = __ballot_sync(0xffffffffu, base + lane < NT && wl[1 + base + lane]);
+        for (; m; m &= m - 1, ++rank) {
+          if (rank % nwarps != warp) continue;
+          const int idx = base + __ffs(m) - 1;
           CellIn c;
           CellWork<float> w;
           w.have = false;
@@ -1089,12 +992,25 @@ __global__ void __launch_bounds__(128) k_admm_small(DevPtrs d, SuParams P, Robot
             } else {
               cell_store(ds, c, o, &hm2, &dual);
             }
-            atomicAdd(&ds.resi_acc[0], hm2);
-            atomicAdd(&ds.resi_acc[1], dual);
+            hm2s += hm2;
+            duals += dual;
             atomicAdd(&d.counters[o.path == CELL_FAILED ? 2 : 1], 1);
           }
           __syncwarp();
         }
+      }
+      for (int o2 = 16; o2 > 0; o2 >>= 1) {
+        hm2s += __shfl_xor_sync(0xffffffffu, hm2s, o2);
+        duals += __shfl_xor_sync(0xffffffffu, duals, o2);
+      }
+      float* part = misc + 16;                       // [warp][2] sums of the (at most 4) warps
+      if (lane == 0) { part[2 * warp] = hm2s; part[2 * warp + 1] = duals; }
+      __syncthreads();
+      if (tid == 0) {
+        float hm2 = 0.f, dual = 0.f;
+        for (int k = 0; k < nwarps; ++k) { hm2 += part[2 * k]; dual += part[2 * k + 1]; }
+        ds.resi_acc[0] = hm2;
+        ds.resi_acc[1] = dual;
       }
     }
     __syncthreads();
@@ -1297,8 +1213,6 @@ int rda_create(const rda_config* cfg, const rda_tunables* tun, rda_handle** out)
     // bulk (TMA) staging needs every staged block to be a multiple of 16 bytes: N*E*T, N*R*T and N*T multiples of 4
     h->small_bulk = (N > 0) && ((N * E * T) % 4 == 0) && ((N * R * T) % 4 == 0) && ((N * T) % 4 == 0);
     if (const char* v = getenv("RDA_B200_SMALL_BULK")) { if (atoi(v) == 0) h->small_bulk = 0; }
-    h->small_coop = 1;
-    if (const char* v = getenv("RDA_B200_SMALL_COOP")) h->small_coop = atoi(v) != 0;
     if (const char* v = getenv("RDA_B200_SMALL")) { int x = atoi(v); if (x >= -1 && x <= 1) h->small_mode = x; }
     if (const char* v = getenv("RDA_B200_SMALL_MAX")) { int x = atoi(v); if (x >= 1) h->small_max = x; }
     if (h->small_ok) {
@@ -1308,21 +1222,8 @@ int rda_create(const rda_config* cfg, const rda_tunables* tun, rda_handle** out)
     }
   }
   if (const char* v = getenv("RDA_B200_SU_PRUNE")) { float x = (float)atof(v); if (x >= 0.f) h->su_prune = x; }
-  h->slow_cpw = RDA_SLOW_CPW; h->slow_ctas = 16;
-  h->slow_adapt = 0;
-  if (const char* v = getenv("RDA_B200_SLOW_ADAPT")) h->slow_adapt = atoi(v) != 0;
-  // one cell per WARP beat one cell per thread at every batch size measured now that only 0.1 % of the cells reach this
-  // pass, BASELINE config C (disc cells on the barrier iteration) most
-  h->slow_coop = 1;
-  if (const char* v = getenv("RDA_B200_SLOW_COOP")) h->slow_coop = atoi(v) != 0;
-  h->dr_coop = 1;
-  if (const char* v = getenv("RDA_B200_DR_COOP")) h->dr_coop = atoi(v) != 0;
   h->extra_min = 3000;
   if (const char* v = getenv("RDA_B200_EXTRA_MIN")) { int x = atoi(v); if (x >= 1) h->extra_min = x; }
-  h->mid_ctas = 16;     // a few waves of the 6 resident CTAs per SM
-  if (const char* v = getenv("RDA_B200_MID_CTAS")) { int x = atoi(v); if (x >= 1 && x <= 64) h->mid_ctas = x; }
-  if (const char* v = getenv("RDA_B200_SLOW_CPW")) { int x = atoi(v); if (x >= 1 && x <= 32) h->slow_cpw = x; }
-  if (const char* v = getenv("RDA_B200_SLOW_CTAS")) { int x = atoi(v); if (x >= 1 && x <= 256) h->slow_ctas = x; }
   if (const char* sm = getenv("RDA_B200_SPLIT_MIN")) { int v = atoi(sm); if (v >= 2) h->split_min = v; }
   if (const char* sp = getenv("RDA_B200_SPLIT_PARTS")) { int v = atoi(sp); if (v >= 1 && v <= 4) h->parts = v; }
   rc = rda_cold_start(h, nullptr);
@@ -1438,14 +1339,11 @@ static int step_lammuz_part(rda_handle* h, int b0, int nb, int part, cudaStream_
     if (h->rb.disc) {
       k_cells_dr<<<grid_for((long long)nb * h->N * h->T, 128, h->sms), 128, 0, s>>>(d, h->rb, h->tun.ro2, theta);
       RDA_CUDA(cudaGetLastError());
-      if (h->dr_coop) {
-        k_cells_dr_mid<<<h->sms * 8, 128, 0, s>>>(d, h->rb, h->tun.ro2, theta);
-        RDA_CUDA(cudaGetLastError());
-        h->launches += 1;
-        k_cells_dr_slow_coop<<<h->sms * 16, 32 * DR_COOP_WARPS, 0, s>>>(d, h->rb, h->tun.ro2, theta);
-      } else k_cells_dr_slow<<<h->sms * 16, 64, 0, s>>>(d, h->rb, h->tun.ro2, theta);
+      k_cells_dr_mid<<<h->sms * 8, 128, 0, s>>>(d, h->rb, h->tun.ro2, theta);
       RDA_CUDA(cudaGetLastError());
-      h->launches += 2;
+      k_cells_dr_slow_coop<<<h->sms * 16, 32 * COOP_WARPS, 0, s>>>(d, h->rb, h->tun.ro2, theta);
+      RDA_CUDA(cudaGetLastError());
+      h->launches += 3;
       k_finalize<<<(nb + 127) / 128, 128, 0, s>>>(d, h->rb, h->iter_threshold);
       RDA_CUDA(cudaGetLastError());
       h->launches += 1;
@@ -1466,19 +1364,16 @@ static int step_lammuz_part(rda_handle* h, int b0, int nb, int part, cudaStream_
     else
       k_cells_fast<8, 8, false><<<grid_for((long long)nb * h->N * h->T, 128, h->sms), 128, 0, s>>>(d, h->rb, theta);
     RDA_CUDA(cudaGetLastError());
-    k_cells_mid<<<h->sms * h->mid_ctas, 128, 0, s>>>(d, h->rb, h->tun.ro2, theta);
+    k_cells_mid<<<h->sms * 16, 128, 0, s>>>(d, h->rb, h->tun.ro2, theta);     // a few waves of the 6 resident CTAs per SM
     RDA_CUDA(cudaGetLastError());
-    if (h->slow_coop) {
-      // the split costs a launch and pays from a few thousand instances on
-      const int split = nb >= h->extra_min;
-      if (split) {
-        k_cells_extra<<<h->sms * 4, 128, 0, s>>>(d, h->rb, h->tun.ro2, theta);
-        RDA_CUDA(cudaGetLastError());
-        h->launches += 1;
-      }
-      k_cells_slow_coop<<<h->sms * h->slow_ctas, 32 * SLOW_COOP_WARPS, 0, s>>>(d, h->rb, h->tun.ro2, theta, split);
+    // the split costs a launch and pays from a few thousand instances on
+    const int split = nb >= h->extra_min;
+    if (split) {
+      k_cells_extra<<<h->sms * 4, 128, 0, s>>>(d, h->rb, h->tun.ro2, theta);
+      RDA_CUDA(cudaGetLastError());
+      h->launches += 1;
     }
-    else k_cells_slow<<<h->sms * h->slow_ctas, 64, 0, s>>>(d, h->rb, h->tun.ro2, theta, h->slow_cpw, h->slow_adapt);
+    k_cells_slow_coop<<<h->sms * 16, 32 * COOP_WARPS, 0, s>>>(d, h->rb, h->tun.ro2, theta, split);
     RDA_CUDA(cudaGetLastError());
     h->launches += 3;
   }
@@ -1564,11 +1459,11 @@ int rda_solve(rda_handle* h, const rda_inputs* in, const rda_outputs* out, int i
     if (h->cfg.su_fp64)
       k_admm_small<double><<<h->B, 128, h->small_L.total, s0>>>(d, P, h->rb, h->tun.ro2, theta, iter_threshold, iter_num, h->small_L,
                                                               (const float*)in->nom_s, (const float*)in->nom_u, (const float*)in->ref_s,
-                                                              (const float*)in->ref_speed, *out, h->small_bulk, h->small_coop);
+                                                              (const float*)in->ref_speed, *out, h->small_bulk);
     else
       k_admm_small<float><<<h->B, 128, h->small_L.total, s0>>>(d, P, h->rb, h->tun.ro2, theta, iter_threshold, iter_num, h->small_L,
                                                              (const float*)in->nom_s, (const float*)in->nom_u, (const float*)in->ref_s,
-                                                             (const float*)in->ref_speed, *out, h->small_bulk, h->small_coop);
+                                                             (const float*)in->ref_speed, *out, h->small_bulk);
     RDA_CUDA(cudaGetLastError());
     h->launches = 1;
     return 0;

@@ -150,7 +150,8 @@ def test_disc_robot_port_matches_committed_oracle_traces(name):
 @pytest.mark.gpu
 @pytest.mark.parametrize('name', ['a', 'b', 'c', 'd', 'e'])
 def test_gpu_disc_robot_matches_committed_oracle_traces(name):
-    """The CUDA path (k_cells_dr / k_cells_dr_slow behind the C ABI) through the phase API, every iteration."""
+    """The CUDA path (k_cells_dr / k_cells_dr_mid / k_cells_dr_slow_coop behind the C ABI) through the phase API, every
+    iteration."""
     from rda_planner_b200.rda_solver import RDA_solver
     m = _gen()
     z = np.load(os.path.join(HERE, 'golden', 'oracle_disc_robot.npz'))

@@ -414,29 +414,3 @@ def test_persistent_small_kernel_equals_streaming_kernels(monkeypatch, kind, mov
     for k in res['0'][2]:
         assert float((res['0'][2][k] - res['1'][2][k]).abs().max()) < (1e-3 if fp64 else 5e-2), k
 
-
-@pytest.mark.parametrize('kind,moving', [('polygon', False), ('circle', True)])
-def test_cooperative_last_pass_equals_thread_per_cell(monkeypatch, kind, moving):
-    """RDA_B200_SLOW_COOP=1 runs the interior point pass with one cell per WARP (coop_ipm.cuh over 32 lanes, problem in shared
-    memory) instead of one cell per thread: the same iteration with the sums taken in a different order, so the trajectories
-    agree to float32 rounding and the per-instance statistics are equal."""
-    from rda_planner_b200.rda_solver import RDA_solver
-    from rda_planner_b200 import _cabi
-    T, N, B = 16, 8, 48
-    monkeypatch.setenv('RDA_B200_SMALL', '0')
-    car = rectangle_robot()
-    insts, inp = _batch_inputs(B, T, N, 2500, lateral=(0.2, 2.5), kind=kind, moving=moving)
-    dev = {k: torch.as_tensor(v, device='cuda', dtype=torch.int32 if 'kind' in k or 'count' in k else torch.float32)
-           for k, v in inp.items()}
-    res = {}
-    for coop in ('0', '1'):
-        monkeypatch.setenv('RDA_B200_SLOW_COOP', coop)
-        g = RDA_solver(T, car, 4, N, iter_num=6, iter_threshold=0.0, time_print=False, batch=B)
-        out = {k: v.clone() for k, v in g.iterative_solve_batch(**dev, time_varying=moving).items()}
-        res[coop] = (out, g.state_buffer(_cabi.BUF_COUNTERS).clone())
-    a, b = res['0'][0], res['1'][0]
-    assert int(res['0'][1][1]) > 0, 'the instances must exercise the interior point pass'
-    assert int(res['0'][1][1]) == int(res['1'][1][1]) and int(res['1'][1][2]) == 0          # same cells, no fall-back
-    assert torch.equal(a['status'], b['status'])
-    assert float((a['s'] - b['s']).abs().max()) < 2e-4 and float((a['u'] - b['u']).abs().max()) < 1e-3
-    assert torch.allclose(a['resi_pri'], b['resi_pri'], rtol=1e-3, atol=1e-5)

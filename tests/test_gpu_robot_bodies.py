@@ -1,6 +1,7 @@
 """-m gpu: polygon robot bodies other than the rear-axle rectangle (tests/golden/make_oracle_fixture_bodies.py) through every
 cell routing the library selects by R: k_cells_fast<4,4> with padded robot rows (R = 3), the coherent pass k_cells_coh at R = 3
-and with outside reference points, k_cells_fast<8,8> at E = 4 (R = 5..8), the persistent kernel's staging of mu blocks of
+and with outside reference points, k_cells_fast<8,8> at E = 4 (R = 5..8), k_cells_extra ahead of the cooperative last pass at
+every R, the persistent kernel's staging of mu blocks of
 N*R*T floats, and the R loops of cell_store / k_reset / k_finalize.  Every cell of a batch against the float64 generic solver,
 whole solves against the committed oracle traces, invariances between the paths, and the order of the body's rows."""
 import os
@@ -21,7 +22,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROUTING_ENV = {                     # environment read by rda_create
     'stream': {'RDA_B200_SMALL': '0'},
     'coherent': {'RDA_B200_SMALL': '0', 'RDA_B200_LEAN2': '1', 'RDA_B200_EXTRA_MIN': '1'},
-    'thread_slow': {'RDA_B200_SMALL': '0', 'RDA_B200_SLOW_COOP': '0'},
+    'extra': {'RDA_B200_SMALL': '0', 'RDA_B200_EXTRA_MIN': '1'},
     'small': {'RDA_B200_SMALL': '1'},
 }
 
@@ -32,7 +33,7 @@ def _R(name):
 
 def _solver(monkeypatch, routing, car, T, N, iters, B=1, env=None):
     from rda_planner_b200.rda_solver import RDA_solver
-    for k in ('RDA_B200_SMALL', 'RDA_B200_LEAN2', 'RDA_B200_EXTRA_MIN', 'RDA_B200_SLOW_COOP', 'RDA_B200_SMALL_BULK'):
+    for k in ('RDA_B200_SMALL', 'RDA_B200_LEAN2', 'RDA_B200_EXTRA_MIN', 'RDA_B200_SMALL_BULK'):
         monkeypatch.delenv(k, raising=False)
     for k, v in {**ROUTING_ENV[routing], **(env or {})}.items():
         monkeypatch.setenv(k, v)
@@ -73,7 +74,7 @@ def _generic(A, b, circ, G, h, p, phi, dbar, zeta, xi, ro2):
     return _GENERIC[key]
 
 
-CELL_CASES = [(n, r) for n in NAMES for r in (('stream', 'coherent', 'thread_slow') if _R(n) <= 4 else ('stream', 'thread_slow'))]
+CELL_CASES = [(n, r) for n in NAMES for r in (('stream', 'coherent', 'extra') if _R(n) <= 4 else ('stream', 'extra'))]
 
 
 @pytest.mark.parametrize('name,routing', CELL_CASES)
@@ -160,6 +161,8 @@ def test_every_cell_equals_generic_solver(monkeypatch, name, routing):
     assert cnt[2] == 0 and cnt[1] > 0                   # the interior point (or extra closed-form) pass saw cells of this body
     if routing == 'coherent':
         assert launches == 7, launches                  # k_cells_coh, listed k_cells_fast and k_cells_extra ran
+    elif routing == 'extra':
+        assert launches == 5, launches                  # k_cells_extra ran, k_cells_slow_coop read its list
     else:
         assert launches == 4, launches
 

@@ -29,7 +29,7 @@ for kind, moving in (('polygon', False), ('circle', True)):
     torch.cuda.synchronize()
     print(kind, 'ok', bool(torch.isfinite(out['u']).all()), int((out['status'] & 6).sum()))
 
-# disc body (cone_type 'norm2'): k_cells_dr / k_cells_dr_slow
+# disc body (cone_type 'norm2'): k_cells_dr / k_cells_dr_mid / k_cells_dr_slow_coop
 from rda_planner_b200.scenarios import disc_robot  # noqa: E402
 T, N, B = 8, 4, 24
 insts = [make_instance(140 + i, T=T, N=N, E=4, kind='polygon' if i % 2 else 'circle', lateral=(0.3, 3.0), dynamics='diff') for i in range(B)]
