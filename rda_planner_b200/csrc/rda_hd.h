@@ -43,12 +43,12 @@ RDA_HD double rcp_(double x) {
   return 1.0 / x;
 #endif
 }
-// index of the lowest set bit (m != 0)
-RDA_HD int ctz_(unsigned m) {
+// number of set bits
+RDA_HD int popc_(unsigned m) {
 #if defined(__CUDA_ARCH__)
-  return __ffs((int)m) - 1;
+  return __popc(m);
 #else
-  return __builtin_ctz(m);
+  return __builtin_popcount(m);
 #endif
 }
 RDA_HD bool finite_(float x) { return isfinite(x); }

@@ -202,7 +202,7 @@ __global__ void __launch_bounds__(32) k_su(DevPtrs d, SuParams P) {
   WarpCtx ctx;
   SuWork<Real> W;
   // per-hinge data stays in global memory (L2): every entry is touched only by the lane that owns
-  // its stage, consecutive lanes read consecutive addresses
+  // its stage, consecutive lanes read consecutive addresses (the compact hinge list: row k of every stage)
   su_work_layout<Real>(P.T, P.N, &W, smem, false, d.su_ws + (size_t)b * d.su_ws_stride);
   su_instance<Real>(d, P, b, W, ctx);
 }
@@ -830,14 +830,15 @@ __global__ void k_finalize(DevPtrs d, RobotGeom rb, float thr) {
 // pointers address shared memory, so the arithmetic is identical; instances progress independently (no grid-wide
 // barrier between the ADMM phases).
 // ------------------------------------------------------------------------------------------------
-static SmallLayout small_layout(int T, int N, int E, int R, size_t su_bytes) {
+// su_bytes, su_gbytes: the su-QP workspace and its per-hinge arrays (su_work_bytes with hinge_arrays = false)
+static SmallLayout small_layout(int T, int N, int E, int R, size_t su_bytes, size_t su_gbytes) {
   SmallLayout L;
   size_t o = 0;
   auto take = [&](size_t bytes) { o = (o + 15) & ~(size_t)15; size_t r = o; o += bytes; return (int)r; };
   const size_t NT = (size_t)N * T;
   L.lam = take(4 * N * E * T); L.mu = take(4 * N * R * T); L.z = take(4 * NT); L.xi = take(8 * NT); L.zeta = take(4 * NT);
   L.dis = take(4 * T); L.coef = take(20 * NT); L.pref = take(8 * T); L.cur_s = take(12 * (T + 1)); L.cur_u = take(8 * T);
-  L.ref_s = take(12 * (T + 1)); L.misc = take(128); L.hs = take(16 * NT); L.su = take(su_bytes);
+  L.ref_s = take(12 * (T + 1)); L.misc = take(128); L.hs = take(su_gbytes); L.su = take(su_bytes);
   // which cells the closed forms left (one flag per cell) and one interior point problem per warp (cooperative pass)
   L.wl = take(4 * (NT + 1)); L.slow = take(4 * sizeof(CellSlowStore));
   L.total = (int)((o + 15) & ~(size_t)15);
@@ -1206,8 +1207,9 @@ int rda_create(const rda_config* cfg, const rda_tunables* tun, rda_handle** out)
   h->parts = 2;
   h->su_prune = 0.5f;       // chosen by a sweep of 0.5, 1, 2 and off at B = 16384
   {
-    const size_t sub = cfg->su_fp64 ? su_work_bytes<double>((int)T, (int)N, false) : su_work_bytes<float>((int)T, (int)N, false);
-    h->small_L = small_layout((int)T, (int)N, (int)E, (int)R, sub);
+    size_t g = 0;
+    const size_t sub = cfg->su_fp64 ? su_work_bytes<double>((int)T, (int)N, false, &g) : su_work_bytes<float>((int)T, (int)N, false, &g);
+    h->small_L = small_layout((int)T, (int)N, (int)E, (int)R, sub, g);
     h->small_ok = h->small_L.total <= 200 * 1024 && !h->rb.disc;      // the persistent kernel has the polygon body's cells only
     h->small_mode = -1; h->small_max = 2 * h->sms;      // two resident CTAs per SM
     // bulk (TMA) staging needs every staged block to be a multiple of 16 bytes: N*E*T, N*R*T and N*T multiples of 4

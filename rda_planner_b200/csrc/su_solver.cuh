@@ -36,8 +36,9 @@ struct SuParams {
                   // the interior point iteration and verified afterwards (accelerated mode only); 0: keep all
 };
 
-// Per-instance workspace.  All arrays indexed by stage t (0..T-1) unless noted; hinge arrays indexed
-// [o*T + t].  Real: arithmetic, iterate and slack / multiplier type.
+// Per-instance workspace.  All arrays indexed by stage t (0..T-1) unless noted; hinge planes (hx, hy, hc) indexed
+// [o*T + t], the compact hinge list (kx, ky, kc, hs, hnu) [k*T + t].  Real: arithmetic, iterate and slack / multiplier
+// type.
 template <typename Real>
 struct SuWork {
   Real *s, *u, *d;            // iterate: 3(T+1), 2T, T
@@ -46,9 +47,12 @@ struct SuWork {
   Real *Aj, *Bj, *Cj;         // 2T (A02, A12), 6T, 3T; Cj is dead after the initial rollout (shares K)
   Real *Skk, *Sgk;            // aggregated rotation-consensus terms
   float *pref;                // 2T positions the hinge offsets refer to
-  float *hx, *hy, *hc;        // hinge rows: lam'A (2) and offset
-  Real *hs, *hnu;             // hinge slack / multiplier
+  float *hx, *hy, *hc;        // hinge rows: lam'A (2) and offset, one plane per obstacle
   unsigned *hmask;            // T x ceil(N/32) words: hinges of stage t that take part in the interior point iteration
+  // Compact list of those hinges: slot k of stage t (k < popcount of its hmask words) holds its k-th kept hinge in
+  // ascending o, so that the lanes of a warp read one contiguous row k in the per-hinge passes.  Rebuilt by every attempt.
+  float *kx, *ky, *kc;        // copies of hx, hy, hc
+  Real *hs, *hnu;             // hinge slack / multiplier
   Real *bs, *bnu;             // 10T box/rate slack / multiplier, entry (t, c) at 10 * t + c
   Real *Wm;                   // 3T hinge Hessian of the position block after the elimination of d_t (xx, xy, yy)
   Real *Ed;                   // 3T elimination of d_t: (M_xd / Q_dd, M_yd / Q_dd, 1 / Q_dd)
@@ -69,8 +73,8 @@ struct SuWork {
 
 // Workspace placement.  `base` is the fast memory of the instance (shared memory on the GPU), `gbase` an
 // optional per-instance slab of global memory (L2).  Everything lives in `base`, except that with
-// hinge_arrays = false the per-hinge arrays (hx, hy, hc: caller; hs, hnu: `gbase`) are left out of it (each
-// entry is touched only by the lane that owns its stage).  Returns the bytes of `base` used; *gbytes the
+// hinge_arrays = false the per-hinge arrays (hx, hy, hc: caller; kx, ky, kc, hs, hnu: `gbase`) are left out of it
+// (each entry is touched only by the lane that owns its stage).  Returns the bytes of `base` used; *gbytes the
 // bytes of `gbase`.
 template <typename Real>
 RDA_HD size_t su_work_layout(int T, int N, SuWork<Real>* w, char* base, bool hinge_arrays = true,
@@ -98,8 +102,10 @@ RDA_HD size_t su_work_layout(int T, int N, SuWork<Real>* w, char* base, bool hin
   if (hinge_arrays) {
     RDA_TAKE_S(hx, N * T, float) RDA_TAKE_S(hy, N * T, float) RDA_TAKE_S(hc, N * T, float)
     RDA_TAKE_S(hs, N * T, Real) RDA_TAKE_S(hnu, N * T, Real)
+    RDA_TAKE_S(kx, N * T, float) RDA_TAKE_S(ky, N * T, float) RDA_TAKE_S(kc, N * T, float)
   } else {
     RDA_TAKE_G(hs, N * T, Real) RDA_TAKE_G(hnu, N * T, Real)
+    RDA_TAKE_G(kx, N * T, float) RDA_TAKE_G(ky, N * T, float) RDA_TAKE_G(kc, N * T, float)
   }
   RDA_TAKE_S(bs, 10 * T, Real) RDA_TAKE_S(bnu, 10 * T, Real)
   RDA_TAKE_S(Wm, 8 * T + 5, Real)                                     // (Wm, wb) | (dza, dva)
@@ -361,6 +367,11 @@ RDA_HD int su_solve(const SuParams& P, SuWork<Real>& W, Ctx& ctx, const float* g
   // (obstacles the robot is far from: ~3/4 of the hinges of the bench workload), so the per-hinge passes — about
   // two thirds of this kernel's time (profiles/ncu_r02_ksu_lines_before.md) — run over the rest only.
   const int NW = (N + 31) / 32 > 0 ? (N + 31) / 32 : 1;
+  auto kept = [&](int t) {                // length of the compact hinge list of stage t
+    int n = 0;
+    for (int w = 0; w < NW; ++w) n += popc_(W.hmask[t * NW + w]);
+    return n;
+  };
   const bool can_prune = acc && N > 0 && P.prune > 0;
   int status = 1, it = 0, it_total = 0;
   W.restarts = 0;
@@ -400,18 +411,23 @@ RDA_HD int su_solve(const SuParams& P, SuWork<Real>& W, Ctx& ctx, const float* g
           const Real lp = (Real)W.hx[o * T + t] * dx + (Real)W.hy[o * T + t] * dy + (Real)W.hc[o * T + t];
           if (lp < lmin1) { lmin2 = lmin1; lmin1 = lp; } else if (lp < lmin2) lmin2 = lp;
         }
+      int k = 0;
       for (int o = 0; o < N; ++o) {
-        const Real lp = (Real)W.hx[o * T + t] * dx + (Real)W.hy[o * T + t] * dy + (Real)W.hc[o * T + t];
+        const float ax = W.hx[o * T + t], ay = W.hy[o * T + t], hc = W.hc[o * T + t];
+        const Real lp = (Real)ax * dx + (Real)ay * dy + (Real)hc;
         if (!full && lp - (Real)P.dmax > (Real)P.prune && lp > lmin2) continue;        // left out, verified after convergence
         W.hmask[t * NW + (o >> 5)] |= 1u << (o & 31);
+        const int i = k++ * T + t;
+        W.kx[i] = ax; W.ky[i] = ay; W.kc[i] = hc;
         Real l = lp - W.d[t];
         Real sv = (l + sqrt_(l * l + 4 * mu0 / ro1)) / 2;
-        W.hs[o * T + t] = sv;
-        W.hnu[o * T + t] = mu0 / sv;
+        W.hs[i] = sv;
+        W.hnu[i] = mu0 / sv;
         ++nrows;
       }
     } else {
       for (int w = 0; w < NW; ++w) W.hmask[t * NW + w] = (N - 32 * w >= 32) ? 0xffffffffu : ((N - 32 * w > 0) ? ((1u << (N - 32 * w)) - 1u) : 0u);
+      for (int o = 0; o < N; ++o) { W.kx[o * T + t] = W.hx[o * T + t]; W.ky[o * T + t] = W.hy[o * T + t]; W.kc[o * T + t] = W.hc[o * T + t]; }
     }
   }
   const Real Mrows = ctx.sum((Real)nrows);
@@ -481,21 +497,18 @@ RDA_HD int su_solve(const SuParams& P, SuWork<Real>& W, Ctx& ctx, const float* g
         // hinges in chunks of RDA_SU_CH: all (global-memory) loads of a chunk are issued before its arithmetic
         const Real adx = phase == 1 ? W.dza[5 * t + 5] : (Real)0, ady = phase == 1 ? W.dza[5 * t + 6] : (Real)0;
         const Real add = phase == 1 ? W.dva[3 * t + 2] : (Real)0;
-        for (int w_ = 0; w_ < NW; ++w_) {
-          unsigned m_ = W.hmask[t * NW + w_];
-          while (m_) {
-          int oi[RDA_SU_CH], cnt_ = 0;
+        const int nk = kept(t);
+        for (int k0 = 0; k0 < nk; k0 += RDA_SU_CH) {
           Real axv[RDA_SU_CH], ayv[RDA_SU_CH], hcv[RDA_SU_CH], svv[RDA_SU_CH], nuv[RDA_SU_CH];
 #pragma unroll
           for (int k = 0; k < RDA_SU_CH; ++k) {
-            if (m_) { oi[k] = (32 * w_ + ctz_(m_)) * T + t; m_ &= m_ - 1u; cnt_ = k + 1; } else oi[k] = oi[0];
-            const int i = oi[k];
-            axv[k] = W.hx[i]; ayv[k] = W.hy[i]; hcv[k] = W.hc[i];
+            const int i = (k0 + k < nk ? k0 + k : k0) * T + t;
+            axv[k] = W.kx[i]; ayv[k] = W.ky[i]; hcv[k] = W.kc[i];
             svv[k] = acc ? (Real)W.hs[i] : (Real)1; nuv[k] = acc ? (Real)W.hnu[i] : (Real)1;
           }
 #pragma unroll
           for (int k = 0; k < RDA_SU_CH; ++k) {
-            if (k >= cnt_) break;
+            if (k0 + k >= nk) break;
             const Real ax = axv[k], ay = ayv[k];
             const Real l = ax * dx + ay * dy + hcv[k] - dd;
             Real tk, om;
@@ -525,7 +538,6 @@ RDA_HD int su_solve(const SuParams& P, SuWork<Real>& W, Ctx& ctx, const float* g
               m0 += om * ax * ax; m1 += om * ax * ay; m2 -= om * ax;
               m3 += om * ay * ay; m4 -= om * ay; m5 += om;
             }
-          }
           }
         }
         // eliminate d_t (it enters stage t only): Schur complement on Q_dd = reg + barrier weights + sum om
@@ -580,20 +592,17 @@ RDA_HD int su_solve(const SuParams& P, SuWork<Real>& W, Ctx& ctx, const float* g
           const Real dx = W.s[3 * t + 3] - W.pref[2 * t], dy = W.s[3 * t + 4] - W.pref[2 * t + 1], dd = W.d[t];
           const Real zdx = dz[5 * t + 5], zdy = dz[5 * t + 6], zdd = dv[3 * t + 2];
           const Real adx = W.dza[5 * t + 5], ady = W.dza[5 * t + 6], add = W.dva[3 * t + 2];
-          for (int w_ = 0; w_ < NW; ++w_) {
-            unsigned m_ = W.hmask[t * NW + w_];
-            while (m_) {
-            int oi[RDA_SU_CH], cnt_ = 0;
+          const int nk = kept(t);
+          for (int k0 = 0; k0 < nk; k0 += RDA_SU_CH) {
             Real axv[RDA_SU_CH], ayv[RDA_SU_CH], hcv[RDA_SU_CH], svv[RDA_SU_CH], nuv[RDA_SU_CH];
 #pragma unroll
             for (int k = 0; k < RDA_SU_CH; ++k) {
-              if (m_) { oi[k] = (32 * w_ + ctz_(m_)) * T + t; m_ &= m_ - 1u; cnt_ = k + 1; } else oi[k] = oi[0];
-              const int i = oi[k];
-              axv[k] = W.hx[i]; ayv[k] = W.hy[i]; hcv[k] = W.hc[i]; svv[k] = W.hs[i]; nuv[k] = W.hnu[i];
+              const int i = (k0 + k < nk ? k0 + k : k0) * T + t;
+              axv[k] = W.kx[i]; ayv[k] = W.ky[i]; hcv[k] = W.kc[i]; svv[k] = W.hs[i]; nuv[k] = W.hnu[i];
             }
 #pragma unroll
             for (int k = 0; k < RDA_SU_CH; ++k) {
-              if (k >= cnt_) break;
+              if (k0 + k >= nk) break;
               const Real ax = axv[k], ay = ayv[k], sv = svv[k], nu = nuv[k];
               const Real l = ax * dx + ay * dy + hcv[k] - dd;
               const Real nr = nu * iro1;
@@ -613,7 +622,6 @@ RDA_HD int su_solve(const SuParams& P, SuWork<Real>& W, Ctx& ctx, const float* g
               const Real ip = rcp_(sv * nu);
               rmaxr = rmax(rmaxr, rmax(-ds * nu * ip, -dn * sv * ip));
               s0 += sv * nu; s1 += sv * dn + nu * ds; s2 += ds * dn;
-            }
             }
           }
         }
@@ -656,20 +664,17 @@ RDA_HD int su_solve(const SuParams& P, SuWork<Real>& W, Ctx& ctx, const float* g
             const Real dx = W.s[3 * t + 3] - W.pref[2 * t], dy = W.s[3 * t + 4] - W.pref[2 * t + 1], dd = W.d[t];
             const Real zdx = W.dz[5 * t + 5], zdy = W.dz[5 * t + 6], zdd = W.dv[3 * t + 2];
             const Real adx = W.dza[5 * t + 5], ady = W.dza[5 * t + 6], add = W.dva[3 * t + 2];
-            for (int w_ = 0; w_ < NW; ++w_) {
-              unsigned m_ = W.hmask[t * NW + w_];
-              while (m_) {
-              int oi[RDA_SU_CH], cnt_ = 0;
+            const int nk = kept(t);
+            for (int k0 = 0; k0 < nk; k0 += RDA_SU_CH) {
               Real axv[RDA_SU_CH], ayv[RDA_SU_CH], hcv[RDA_SU_CH], svv[RDA_SU_CH], nuv[RDA_SU_CH];
 #pragma unroll
               for (int k = 0; k < RDA_SU_CH; ++k) {
-                if (m_) { oi[k] = (32 * w_ + ctz_(m_)) * T + t; m_ &= m_ - 1u; cnt_ = k + 1; } else oi[k] = oi[0];
-                const int i = oi[k];
-                axv[k] = W.hx[i]; ayv[k] = W.hy[i]; hcv[k] = W.hc[i]; svv[k] = W.hs[i]; nuv[k] = W.hnu[i];
+                const int i = (k0 + k < nk ? k0 + k : k0) * T + t;
+                axv[k] = W.kx[i]; ayv[k] = W.ky[i]; hcv[k] = W.kc[i]; svv[k] = W.hs[i]; nuv[k] = W.hnu[i];
               }
 #pragma unroll
               for (int k = 0; k < RDA_SU_CH; ++k) {
-                if (k >= cnt_) break;
+                if (k0 + k >= nk) break;
                 const Real ax = axv[k], ay = ayv[k], sv = svv[k], nu = nuv[k];
                 const Real l = ax * dx + ay * dy + hcv[k] - dd;
                 const Real nr = nu * iro1;
@@ -683,9 +688,8 @@ RDA_HD int su_solve(const SuParams& P, SuWork<Real>& W, Ctx& ctx, const float* g
                 const Real cc = sv * nu - sigma_mu + dsa * dna;
                 const Real dn = -(cc + nu * res + nu * dir) * iden;
                 const Real ds = dir + dn * iro1 + res;
-                W.hs[oi[k]] = sv + a * ds;
-                W.hnu[oi[k]] = nu + a * dn;
-              }
+                W.hs[(k0 + k) * T + t] = sv + a * ds;
+                W.hnu[(k0 + k) * T + t] = nu + a * dn;
               }
             }
           }
