@@ -25,6 +25,19 @@ struct SmallLayout {
   int lam, mu, z, xi, zeta, dis, coef, pref, cur_s, cur_u, ref_s, misc, hs, su, wl, slow, total;
 };
 
+// A cell a polygon pass declined, handed to the next pass: every value the cell's arithmetic reads from the state planes
+// besides the obstacle rows.  Consecutive list entries are cells of unrelated instances, so gathering them again from the
+// t-fastest planes would cost one 32-byte sector per scalar; a record is five 16-byte loads, consecutive across the warp.
+// The previous duals (dual residual) are in the record when E <= 4 and R <= 4 (rec_duals); otherwise cell_store reads them
+// from the planes.
+struct __align__(16) CellRec {
+  int cell, kind;                                    // b * N * T + o * T + t of the sub-batch, obstacle kind
+  float px, py, cp, sp, dbar, zeta, xi0, xi1;        // as CellIn
+  float lam[4], mu[4], z;                            // previous lam, mu, z of the cell
+  int pad_;
+};
+static_assert(sizeof(CellRec) == 80, "CellRec: five 16-byte words");
+
 struct rda_handle {
   rda_config cfg;
   rda_tunables tun;
@@ -34,6 +47,9 @@ struct rda_handle {
   float *lam, *mu, *z, *xi, *zeta, *dis, *coef, *pref, *cur_s, *cur_u, *ref_s, *ref_speed;
   float *resi_acc, *resi_pri, *resi_dual;
   int *status, *iters, *done, *counters, *worklist, *worklist2;
+  // the declined cells of the polygon passes as records, two lists of B * N * T (every cell may be declined: the cold
+  // start's first iteration has no support-vertex pairs), used in turn (step_lammuz_part)
+  CellRec *rec_a, *rec_b;
   char* su_ws;           // [B][su_ws_stride] global workspace of the su-QP interior point iteration (hinge slacks /
                          // multipliers)
   size_t su_ws_stride;
@@ -42,7 +58,6 @@ struct rda_handle {
   RobotAux ra;
   ObstacleGeom<4>* ogeo; // [B][N] per-obstacle geometry, rebuilt by every rda_begin / rda_solve
   unsigned char* feat;   // [B][N][T] support-vertex pair of the previous iteration (0: none)
-  int* worklist0;        // cells the coherent pass declined (run through the search pass)
   float* rot;            // [B][2][T] cos / sin of the nominal headings of this iteration
   const float *obs_A, *obs_b;
   const int *obs_kind, *obs_count;
@@ -95,7 +110,7 @@ struct DevPtrs {
   int* wl_count;         // lengths of the worklists of this sub-batch ([2]: cells declined by the coherent pass)
   const ObstacleGeom<4>* ogeo;
   unsigned char* feat;
-  int* worklist0;
+  CellRec *rec_a, *rec_b;  // record lists of the polygon cell passes (ping-pong, step_lammuz_part)
   char* su_ws;
   size_t su_ws_stride;
   const float *obs_A, *obs_b;
@@ -215,6 +230,15 @@ struct CellIn {
   const float *A, *bb;
 };
 
+// the obstacle rows of cell (b, o, t) (as cell_load)
+__device__ __forceinline__ void cell_rows(const DevPtrs& d, CellIn& c) {
+  const int tc = d.obs_tv ? (c.t + 1) : 0;
+  const int Tc = d.obs_tv ? (d.T + 1) : 1;
+  const size_t ob = ((size_t)c.b * d.N + c.o) * Tc + tc;
+  c.A = d.obs_A + ob * d.E * 2;
+  c.bb = d.obs_b + ob * d.E;
+}
+
 __device__ __forceinline__ CellIn cell_load(const DevPtrs& d, long long idx) {
   const int T = d.T, N = d.N, E = d.E, NT = N * T;
   CellIn c;
@@ -238,27 +262,83 @@ __device__ __forceinline__ CellIn cell_load(const DevPtrs& d, long long idx) {
   return c;
 }
 
-// write (lam, mu, z), the multiplier updates and the next su-QP's hinge inputs of one cell
+__device__ __forceinline__ bool rec_duals(const DevPtrs& d) { return d.E <= 4 && d.R <= 4; }
+
+__device__ __forceinline__ CellRec cell_rec(const CellIn& c) {
+  CellRec r;
+  r.cell = (int)c.cell; r.kind = c.kind;
+  r.px = c.px; r.py = c.py; r.cp = c.cp; r.sp = c.sp; r.dbar = c.dbar; r.zeta = c.zeta; r.xi0 = c.xi0; r.xi1 = c.xi1;
+  r.pad_ = 0;
+  return r;
+}
+
+__device__ __forceinline__ CellIn cell_from_rec(const DevPtrs& d, const CellRec& r) {
+  const int T = d.T, NT = d.N * T;
+  CellIn c;
+  c.cell = (size_t)r.cell;
+  c.b = r.cell / NT;
+  const int rem = r.cell - c.b * NT;
+  c.o = rem / T; c.t = rem - c.o * T;
+  c.kind = r.kind;
+  c.px = r.px; c.py = r.py; c.cp = r.cp; c.sp = r.sp; c.dbar = r.dbar; c.zeta = r.zeta; c.xi0 = r.xi0; c.xi1 = r.xi1;
+  cell_rows(d, c);
+  return c;
+}
+
+// the record of a cell the whole-batch pass declined, gathered again (from cache: the pass has just read the same values)
+// rather than kept in registers through the cell's arithmetic
+__device__ __forceinline__ CellRec cell_rec_load(const DevPtrs& d, long long idx) {
+  const CellIn c = cell_load(d, idx);
+  CellRec r = cell_rec(c);
+  const int T = d.T, N = d.N, E = d.E, R = d.R;
+  const float* lam = d.lam + ((size_t)c.b * N + c.o) * E * T + c.t;
+  const float* mu = d.mu + ((size_t)c.b * N + c.o) * R * T + c.t;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    r.lam[i] = i < E ? lam[(size_t)i * T] : 0.f;
+    r.mu[i] = i < R ? mu[(size_t)i * T] : 0.f;
+  }
+  r.z = d.z[c.cell];
+  return r;
+}
+
+// the slot in `list` of the record of each lane with `need` set (one atomic per warp on *count), nullptr for the others.
+// A pass that declines a listed cell copies its record over (from cache) instead of keeping it in registers through the
+// cell's arithmetic.
+__device__ __forceinline__ CellRec* rec_slot(bool need, CellRec* list, int* count) {
+  const int lane = threadIdx.x & 31;
+  const unsigned m = __ballot_sync(0xffffffffu, need);
+  if (!m) return nullptr;
+  const int leader = __ffs(m) - 1;
+  int pos = 0;
+  if (lane == leader) pos = atomicAdd(count, __popc(m));
+  pos = __shfl_sync(0xffffffffu, pos, leader);
+  return need ? list + pos + __popc(m & ((1u << lane) - 1)) : nullptr;
+}
+
+// write (lam, mu, z), the multiplier updates and the next su-QP's hinge inputs of one cell; prev: the cell's record, whose
+// previous duals replace the planes' (the same values: a cell's duals are written only by the pass that resolves it)
 __device__ __forceinline__ void cell_store(const DevPtrs& d, const CellIn& c, const CellOut<float>& out, float* hm2,
-                                           float* dual) {
+                                           float* dual, const CellRec* prev = nullptr) {
   const int T = d.T, N = d.N, E = d.E, R = d.R, NT = N * T;
+  const bool pr = prev != nullptr && rec_duals(d);
   // dual residual |lam - lam_prev|^2 + |mu - mu_prev|^2 + |z - z_prev|^2 (:783-787)
   float* lam = d.lam + ((size_t)c.b * N + c.o) * E * T + c.t;
   float acc = 0.f;
   for (int i = 0; i < E; ++i) {
     float nv = out.lam[i];
-    float df = nv - lam[(size_t)i * T];
+    float df = nv - (pr ? prev->lam[i] : lam[(size_t)i * T]);
     acc += df * df;
     lam[(size_t)i * T] = nv;
   }
   float* mu = d.mu + ((size_t)c.b * N + c.o) * R * T + c.t;
   for (int j = 0; j < R; ++j) {
     float nv = out.mu[j];
-    float df = nv - mu[(size_t)j * T];
+    float df = nv - (pr ? prev->mu[j] : mu[(size_t)j * T]);
     acc += df * df;
     mu[(size_t)j * T] = nv;
   }
-  float dz = out.z - d.z[c.cell];
+  float dz = out.z - (prev != nullptr ? prev->z : d.z[c.cell]);
   acc += dz * dz;
   d.z[c.cell] = out.z;
   *dual = acc;
@@ -280,7 +360,8 @@ __device__ __forceinline__ void cell_store(const DevPtrs& d, const CellIn& c, co
 }
 
 // First pass: compile-time specialised lean solver (cell_lean.cuh), geometry in registers.
-// LISTED: the cells come from worklist0 (what the coherent pass k_cells_coh declined) instead of the whole batch.
+// LISTED: the cells come from the records in d.rec_a (what the coherent pass k_cells_coh declined) instead of the whole
+// batch.  What this pass declines goes to d.rec_b as records.
 template <int EC, int RC, bool LISTED>
 __global__ void __launch_bounds__(128, (EC <= 4 ? 6 : 3)) k_cells_fast(DevPtrs d, RobotGeom rb, float theta) {
   const int T = d.T, N = d.N, E = d.E, R = d.R;
@@ -288,15 +369,17 @@ __global__ void __launch_bounds__(128, (EC <= 4 ? 6 : 3)) k_cells_fast(DevPtrs d
   const long long total = LISTED ? (long long)d.wl_count[2] : (long long)d.B * NT;
   const int lane = threadIdx.x & 31;
   for (long long base = (long long)blockIdx.x * blockDim.x; base < total; base += (long long)gridDim.x * blockDim.x) {
-    long long idx = base + threadIdx.x;
+    const long long wi = base + threadIdx.x;
+    long long idx = wi;
     bool live = idx < total;
-    if (LISTED && live) idx = d.worklist0[idx];
+    CellRec rec;
+    if (LISTED && live) { rec = d.rec_a[wi]; idx = rec.cell; }      // listed cells are of live instances (k_cells_coh)
     int b = live ? (int)(idx / NT) : -1;
     float dual = 0.f;
     bool need = false;
-    if (live && (d.done[b] || d.obs_count[b] == 0)) live = false;
+    if (!LISTED && live && (d.done[b] || d.obs_count[b] == 0)) live = false;
     if (live) {
-      CellIn c = cell_load(d, idx);
+      CellIn c = LISTED ? cell_from_rec(d, rec) : cell_load(d, idx);
       // issue every global load of this cell before the arithmetic (memory-level parallelism): the
       // obstacle rows (128-bit loads when E == 4) and the previous duals needed for the residual
       float Ar[2 * EC], br[EC], lamo[EC], muo[RC];
@@ -315,13 +398,22 @@ __global__ void __launch_bounds__(128, (EC <= 4 ? 6 : 3)) k_cells_fast(DevPtrs d
           br[i] = (i < E) ? __ldg(c.bb + i) : 0.f;
         }
       }
-      const float* lamp = d.lam + ((size_t)c.b * N + c.o) * E * T + c.t;
-      const float* mup = d.mu + ((size_t)c.b * N + c.o) * R * T + c.t;
+      float zo;
+      if (LISTED) {            // EC == RC == 4 (E <= 4, R <= 4): the previous duals are in the record
 #pragma unroll
-      for (int i = 0; i < EC; ++i) lamo[i] = (i < E) ? lamp[(size_t)i * T] : 0.f;
+        for (int i = 0; i < EC; ++i) lamo[i] = (i < E) ? rec.lam[i % 4] : 0.f;
 #pragma unroll
-      for (int j = 0; j < RC; ++j) muo[j] = (j < R) ? mup[(size_t)j * T] : 0.f;
-      const float zo = d.z[c.cell];
+        for (int j = 0; j < RC; ++j) muo[j] = (j < R) ? rec.mu[j % 4] : 0.f;
+        zo = rec.z;
+      } else {
+        const float* lamp = d.lam + ((size_t)c.b * N + c.o) * E * T + c.t;
+        const float* mup = d.mu + ((size_t)c.b * N + c.o) * R * T + c.t;
+#pragma unroll
+        for (int i = 0; i < EC; ++i) lamo[i] = (i < E) ? lamp[(size_t)i * T] : 0.f;
+#pragma unroll
+        for (int j = 0; j < RC; ++j) muo[j] = (j < R) ? mup[(size_t)j * T] : 0.f;
+        zo = d.z[c.cell];
+      }
       LeanOut<EC, RC> o;
       const bool ok = cell_lean<EC, RC>(rb, c.kind, EC, Ar, br, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0,
                                         c.xi1, theta, o);
@@ -363,14 +455,8 @@ __global__ void __launch_bounds__(128, (EC <= 4 ? 6 : 3)) k_cells_fast(DevPtrs d
         need = true;
       }
     }
-    // worklist of cells for the second pass (one atomic per warp)
-    unsigned nm = __ballot_sync(0xffffffffu, need);
-    if (nm) {
-      int leader = __ffs(nm) - 1, pos = 0;
-      if (lane == leader) pos = atomicAdd(&d.wl_count[0], __popc(nm));
-      pos = __shfl_sync(0xffffffffu, pos, leader);
-      if (need) d.worklist[pos + __popc(nm & ((1u << lane) - 1))] = (int)idx;
-    }
+    // the records of the cells for the second pass (one atomic per warp)
+    if (CellRec* s = rec_slot(need, d.rec_b, &d.wl_count[0])) *s = LISTED ? d.rec_a[wi] : cell_rec_load(d, idx);
     const bool solved = live && !need;
     // dual-residual partial sums (Hm = 0 for every cell solved here): a warp spans at most two
     // instances when N*T >= 32
@@ -425,7 +511,7 @@ __global__ void k_heading(DevPtrs d, float* rot) {
 }
 
 // Coherent first pass (cell_lean2.cuh): one thread per cell tries the support-vertex pair of the previous
-// iteration; what it declines goes to worklist0 and through k_cells_fast<.., LISTED>.  Grid: one-dimensional,
+// iteration; what it declines goes to d.rec_a as records and through k_cells_fast<.., LISTED>.  Grid: one-dimensional,
 // `tiles` = ceil(cells of one instance / 128) CTAs per instance, instance-major (blockIdx.x = b * tiles + tile,
 // so any batch size fits; gridDim.y would cap it at 65 535) — no 64-bit index arithmetic, one instance per CTA
 // (uniform early exit, one residual atomic per warp), 32-bit offsets inside the instance.
@@ -440,6 +526,7 @@ __global__ void __launch_bounds__(128, 6) k_cells_coh(DevPtrs d, RobotGeom rb, R
   const bool live = rem < NT;
   float dual = 0.f;
   bool need = false, solved = false;
+  CellRec rec;
   if (live) {
     int o = (int)(((float)rem + 0.5f) * invT);
     int t = rem - o * T;
@@ -452,20 +539,21 @@ __global__ void __launch_bounds__(128, 6) k_cells_coh(DevPtrs d, RobotGeom rb, R
     float* zb = d.z + ib * NT;
     float* zetab = d.zeta + ib * NT;
     unsigned char* featb = d.feat + ib * NT;
+    // every input of the cell, read coalesced here: a declined cell takes them to the later passes as its record
     const float xi0 = xi[rem], xi1 = xi[NT + rem];
     const int f = featb[rem];
+    const float px = cs[t + 1], py = cs[(T + 1) + t + 1];
+    const float cp = rot[ib * 2 * T + t], sp = rot[ib * 2 * T + T + t];
+    const float dbar = d.dis[ib * T + t], zeta = zetab[rem];
+    const int lo = o * E * T + t, mo = o * R * T + t;
+    float lamo[EC], muo[RC];
+#pragma unroll
+    for (int i = 0; i < EC; ++i) lamo[i] = (i < E) ? lamb[lo + i * T] : 0.f;
+#pragma unroll
+    for (int j = 0; j < RC; ++j) muo[j] = (j < R) ? mub[mo + j * T] : 0.f;
+    const float zo = zb[rem];
     int nf = -1;
     if (xi0 == 0.f && xi1 == 0.f && (f & RDA_FEAT_VALID)) {
-      const float px = cs[t + 1], py = cs[(T + 1) + t + 1];
-      const float cp = rot[ib * 2 * T + t], sp = rot[ib * 2 * T + T + t];
-      const float dbar = d.dis[ib * T + t], zeta = zetab[rem];
-      const int lo = o * E * T + t, mo = o * R * T + t;
-      float lamo[EC], muo[RC];
-#pragma unroll
-      for (int i = 0; i < EC; ++i) lamo[i] = (i < E) ? lamb[lo + i * T] : 0.f;
-#pragma unroll
-      for (int j = 0; j < RC; ++j) muo[j] = (j < R) ? mub[mo + j * T] : 0.f;
-      const float zo = zb[rem];
       const ObstacleGeom<4>& og = d.ogeo[ib * N + o];         // same address for the T cells of an obstacle
       LeanOut<EC, RC> r;
       nf = cell_lean2<EC, RC>(rb, ra, og, f, px, py, cp, sp, dbar, zeta, theta, r);
@@ -495,15 +583,15 @@ __global__ void __launch_bounds__(128, 6) k_cells_coh(DevPtrs d, RobotGeom rb, R
       }
     }
     need = nf < 0;
+    if (need) {
+      rec.cell = b * NT + rem; rec.kind = d.obs_kind[ib * N + o];
+      rec.px = px; rec.py = py; rec.cp = cp; rec.sp = sp; rec.dbar = dbar; rec.zeta = zeta; rec.xi0 = xi0; rec.xi1 = xi1;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) { rec.lam[i] = lamo[i]; rec.mu[i] = muo[i]; }
+      rec.z = zo; rec.pad_ = 0;
+    }
   }
-  const unsigned nm = __ballot_sync(0xffffffffu, need);
-  if (nm) {
-    const int leader = __ffs(nm) - 1;
-    int pos = 0;
-    if (lane == leader) pos = atomicAdd(&d.wl_count[2], __popc(nm));
-    pos = __shfl_sync(0xffffffffu, pos, leader);
-    if (need) d.worklist0[pos + __popc(nm & ((1u << lane) - 1))] = b * NT + rem;
-  }
+  if (CellRec* s = rec_slot(need, d.rec_a, &d.wl_count[2])) *s = rec;
   const unsigned fast = __ballot_sync(0xffffffffu, solved);
   if (fast) {
     float q = dual;
@@ -534,8 +622,8 @@ __device__ __forceinline__ void rows_preload(const DevPtrs& d, const CellIn& c, 
   }
 }
 
-// Second pass: the searched closed forms (vertex / edge contact, overlap cases) for the cells of the
-// first worklist, one thread per entry; what is still unresolved goes to the second worklist.
+// Second pass: the searched closed forms (vertex / edge contact, overlap cases) for the cells the first pass declined (records
+// in d.rec_b), one thread per record; the records of what is still unresolved go to d.rec_a.
 __global__ void __launch_bounds__(128) k_cells_mid(DevPtrs d, RobotGeom rb, float ro2, float theta) {
   const int count = d.wl_count[0];
   const int lane = threadIdx.x & 31;
@@ -543,10 +631,8 @@ __global__ void __launch_bounds__(128) k_cells_mid(DevPtrs d, RobotGeom rb, floa
     const int wi = base + threadIdx.x;
     const bool live = wi < count;
     bool need = false;
-    long long idx = 0;
     if (live) {
-      idx = d.worklist[wi];
-      CellIn c = cell_load(d, idx);
+      CellIn c = cell_from_rec(d, d.rec_b[wi]);
       RowsLocal rows;
       rows_preload(d, c, rows);
       CellWork<float> w;
@@ -555,20 +641,14 @@ __global__ void __launch_bounds__(128) k_cells_mid(DevPtrs d, RobotGeom rb, floa
         CellOut<float> out;
         cell_back<float>(rb, w, c.zeta, theta, out);
         float hm2 = 0.f, dual = 0.f;
-        cell_store(d, c, out, &hm2, &dual);
+        cell_store(d, c, out, &hm2, &dual, d.rec_b + wi);
         atomicAdd(&d.resi_acc[2 * c.b], hm2);
         atomicAdd(&d.resi_acc[2 * c.b + 1], dual);
       } else {
         need = true;
       }
     }
-    unsigned m = __ballot_sync(0xffffffffu, need);
-    if (m) {
-      int leader = __ffs(m) - 1, pos = 0;
-      if (lane == leader) pos = atomicAdd(&d.wl_count[1], __popc(m));
-      pos = __shfl_sync(0xffffffffu, pos, leader);
-      if (need) d.worklist2[pos + __popc(m & ((1u << lane) - 1))] = (int)idx;
-    }
+    if (CellRec* s = rec_slot(need, d.rec_a, &d.wl_count[1])) *s = d.rec_b[wi];
     unsigned solved = __ballot_sync(0xffffffffu, live && !need);
     if (lane == 0 && solved) atomicAdd(&d.counters[0], __popc(solved));
   }
@@ -703,19 +783,16 @@ __global__ void __launch_bounds__(32 * COOP_WARPS) k_cells_dr_slow_coop(DevPtrs 
 
 // Last pass, first half (with the cooperative interior point pass): the closed forms only the rare cells need (robot edge x
 // obstacle edge, weighted maxima on monotone edges: cell_front<EXTRA>) for the cells the searched pass listed, one THREAD per
-// cell — they resolve ~90 % of that list; what is left (~0.01 % of all cells) goes to k_cells_slow_coop through d.worklist,
-// which the searched pass has consumed by now.  (Doing these closed forms in lane 0 of the cooperative kernel was slow at
+// cell — they resolve ~90 % of that list; the records of what is left (~0.01 % of all cells) go to k_cells_slow_coop through
+// d.rec_b, which the searched pass has consumed by now.  (Doing these closed forms in lane 0 of the cooperative kernel was slow at
 // 16 384 unique instances: ten thousand warps each waiting for one serial lane.)
 __global__ void __launch_bounds__(128) k_cells_extra(DevPtrs d, RobotGeom rb, float ro2, float theta) {
   const int count = d.wl_count[1];
-  const int lane = threadIdx.x & 31;
   for (int base = blockIdx.x * blockDim.x; base < count; base += gridDim.x * blockDim.x) {
     const int wi = base + threadIdx.x;
     bool need = false;
-    int idx = 0;
     if (wi < count) {
-      idx = d.worklist2[wi];
-      CellIn c = cell_load(d, idx);
+      CellIn c = cell_from_rec(d, d.rec_a[wi]);
       RowsLocal rows;
       rows_preload(d, c, rows);
       CellWork<float> w;
@@ -724,7 +801,7 @@ __global__ void __launch_bounds__(128) k_cells_extra(DevPtrs d, RobotGeom rb, fl
         CellOut<float> out;
         cell_back<float>(rb, w, c.zeta, theta, out);
         float hm2 = 0.f, dual = 0.f;
-        cell_store(d, c, out, &hm2, &dual);
+        cell_store(d, c, out, &hm2, &dual, d.rec_a + wi);
         atomicAdd(&d.resi_acc[2 * c.b], hm2);
         atomicAdd(&d.resi_acc[2 * c.b + 1], dual);
         atomicAdd(&d.counters[1], 1);
@@ -732,13 +809,7 @@ __global__ void __launch_bounds__(128) k_cells_extra(DevPtrs d, RobotGeom rb, fl
         need = true;
       }
     }
-    const unsigned m = __ballot_sync(0xffffffffu, need);
-    if (m) {
-      int leader = __ffs(m) - 1, pos = 0;
-      if (lane == leader) pos = atomicAdd(&d.wl_count[4], __popc(m));
-      pos = __shfl_sync(0xffffffffu, pos, leader);
-      if (need) d.worklist[pos + __popc(m & ((1u << lane) - 1))] = idx;
-    }
+    if (CellRec* s = rec_slot(need, d.rec_b, &d.wl_count[4])) *s = d.rec_a[wi];
   }
 }
 
@@ -748,20 +819,19 @@ __global__ void __launch_bounds__(128) k_cells_extra(DevPtrs d, RobotGeom rb, fl
 // instances, three waves of warps) the pass is a pure latency tail, which is what cooperation shortens (DESIGN.md §3.1).
 __global__ void __launch_bounds__(32 * COOP_WARPS) k_cells_slow_coop(DevPtrs d, RobotGeom rb, float ro2, float theta, int from_extra) {
   __shared__ CellSlowStore store[COOP_WARPS];
-  // from_extra: the list k_cells_extra left — d.worklist (the searched pass' list, consumed by now) with its own counter;
-  // otherwise the searched pass' own leftovers (small batches: one launch less, lane 0 runs the EXTRA closed forms)
+  // from_extra: the records k_cells_extra left — d.rec_b (the first pass' list, consumed by now) with its own counter;
+  // otherwise the searched pass' own leftovers in d.rec_a (small batches: one launch less, lane 0 runs the EXTRA closed forms)
   const int count = from_extra ? d.wl_count[4] : d.wl_count[1];
-  const int* list = from_extra ? d.worklist : d.worklist2;
+  const CellRec* list = from_extra ? d.rec_b : d.rec_a;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   CellSlowStore& S = store[warp];
   WarpCtx ctx;
   for (int wi = blockIdx.x * COOP_WARPS + warp; wi < count; wi += gridDim.x * COOP_WARPS) {
-    const long long idx = list[wi];
     CellIn c;
     CellWork<float> w;
     w.have = false;
     if (lane == 0) {
-      c = cell_load(d, idx);
+      c = cell_from_rec(d, list[wi]);
       cell_front<float, false, true>(rb, c.kind, d.E, c.A, c.bb, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0, c.xi1, ro2, w);
     }
     const int have = __shfl_sync(0xffffffffu, (int)w.have, 0);
@@ -778,7 +848,7 @@ __global__ void __launch_bounds__(32 * COOP_WARPS) k_cells_slow_coop(DevPtrs d, 
         dual = INFINITY;
         atomicOr(&d.status[c.b], RDA_ST_CELL_FALLBACK);
       } else {
-        cell_store(d, c, out, &hm2, &dual);
+        cell_store(d, c, out, &hm2, &dual, list + wi);
       }
       atomicAdd(&d.resi_acc[2 * c.b], hm2);
       atomicAdd(&d.resi_acc[2 * c.b + 1], dual);
@@ -1102,7 +1172,8 @@ DevPtrs dev_ptrs(const rda_handle* h, int b0, int nb, int part) {
   d.counters = h->counters; d.wl_count = h->counters + 8 + 8 * part;     // part < 4, 8 counters each
   d.ogeo = h->ogeo ? h->ogeo + o * N : nullptr;
   d.feat = h->feat ? h->feat + o * NT : nullptr;
-  d.worklist0 = h->worklist0 ? h->worklist0 + o * NT : nullptr;
+  d.rec_a = h->rec_a ? h->rec_a + o * NT : nullptr;
+  d.rec_b = h->rec_b ? h->rec_b + o * NT : nullptr;
   d.worklist = h->worklist + o * NT; d.worklist2 = h->worklist2 + o * NT;
   d.su_ws = h->su_ws + o * h->su_ws_stride; d.su_ws_stride = h->su_ws_stride;
   d.obs_A = h->obs_A ? h->obs_A + o * N * Tc * E * 2 : nullptr;
@@ -1180,6 +1251,10 @@ int rda_create(const rda_config* cfg, const rda_tunables* tun, rda_handle** out)
   alloc((float**)&h->counters, 64);     // [0..7] statistics, [8 + 8 part ..] worklist lengths of the sub-batches
   alloc((float**)&h->worklist, B * NT);
   alloc((float**)&h->worklist2, B * NT);
+  if (!h->rb.disc) {     // the disc body's passes list cell indices (worklist, worklist2)
+    alloc((float**)&h->rec_a, B * NT * (sizeof(CellRec) / 4));
+    alloc((float**)&h->rec_b, B * NT * (sizeof(CellRec) / 4));
+  }
   alloc((float**)&h->su_ws, B * (h->su_ws_stride / 4));
   if (e != cudaSuccess) { rda_destroy(h); return (int)e; }
   e = cfg->su_fp64 ? cudaFuncSetAttribute(k_su<double>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)
@@ -1199,7 +1274,6 @@ int rda_create(const rda_config* cfg, const rda_tunables* tun, rda_handle** out)
     robot_aux_from_geom(h->rb, &h->ra);
     e = cudaMalloc((void**)&h->ogeo, B * N * sizeof(ObstacleGeom<4>));
     if (e == cudaSuccess) e = cudaMalloc((void**)&h->feat, B * NT ? B * NT : 1);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&h->worklist0, (B * NT ? B * NT : 1) * sizeof(int));
     if (e == cudaSuccess) e = cudaMalloc((void**)&h->rot, B * 2 * T * sizeof(float));
     if (e != cudaSuccess) { rda_destroy(h); return (int)e; }
   }
@@ -1244,7 +1318,8 @@ int rda_destroy(rda_handle* h) {
   for (float* p : bufs) if (p) cudaFree(p);
   if (h->ogeo) cudaFree(h->ogeo);
   if (h->feat) cudaFree(h->feat);
-  if (h->worklist0) cudaFree(h->worklist0);
+  if (h->rec_a) cudaFree(h->rec_a);
+  if (h->rec_b) cudaFree(h->rec_b);
   if (h->rot) cudaFree(h->rot);
   if (h->ev_fork) cudaEventDestroy(h->ev_fork);
   for (int p = 0; p < 3; ++p) {
