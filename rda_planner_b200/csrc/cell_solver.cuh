@@ -130,11 +130,9 @@ struct CellWork {
 };
 
 // ---- stage 1: geometry relative to the robot reference point and the closed-form cases ----------
-// LEAN = true stops after the two cases that need no search (xi = 0 and a non-negative margin): the
-// first pass of the GPU pipeline, kept small so that its code stays resident in the instruction cache.
 // EXTRA: also try the candidates that only the (rare) cells of the last pass need: robot edge against obstacle edge.
 // The searched pass leaves them out (every one of its cells would pay for the extra candidates, r02 measurement).
-template <typename Real, bool LEAN = false, bool EXTRA = false>
+template <typename Real, bool EXTRA = false>
 RDA_HD void cell_front(const RobotGeom& rb, int kind, int E, const float* A, const float* b, Real px, Real py,
                        Real cphi, Real sphi, Real dbar, Real zeta, Real xi0, Real xi1, Real ro2,
                        CellWork<Real>& w) {
@@ -288,11 +286,6 @@ RDA_HD void cell_front(const RobotGeom& rb, int kind, int E, const float* A, con
   if (!have && !sep && xi_zero && k0 <= 0) {
     // overlapping sets, no tilt: max margin is 0 at v = 0 (stuff = -k0 >= 0)
     exact_zero_q = true; have = true; RDA_CASE_STAT(__LINE__); path = CELL_OVERLAP_FREE;
-  }
-  if (LEAN) {
-    w.v0 = v0; w.v1 = v1; w.g0 = g0; w.g1 = g1;
-    w.exact_zero_q = exact_zero_q; w.have = have; w.path = path;
-    return;
   }
   if (!have && sep) {
     const Real tolc = sizeof(Real) == 4 ? (Real)1e-5 : (Real)1e-11;
@@ -861,7 +854,7 @@ RDA_HD void cell_solve(const RobotGeom& rb, int kind, int E, const float* A, con
                        Real px, Real py, Real cphi, Real sphi, Real dbar, Real zeta, Real xi0,
                        Real xi1, Real ro2, Real theta, CellOut<Real>& out) {
   CellWork<Real> w;
-  cell_front<Real, false, true>(rb, kind, E, A, b, px, py, cphi, sphi, dbar, zeta, xi0, xi1, ro2, w);
+  cell_front<Real, true>(rb, kind, E, A, b, px, py, cphi, sphi, dbar, zeta, xi0, xi1, ro2, w);
   if (!w.have) {
     CellSlowStore S;
     SeqCtx ctx;

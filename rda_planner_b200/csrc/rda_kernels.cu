@@ -25,7 +25,7 @@ struct SmallLayout {
   int lam, mu, z, xi, zeta, dis, coef, pref, cur_s, cur_u, ref_s, misc, hs, su, wl, slow, total;
 };
 
-// A cell a polygon pass declined, handed to the next pass: every value the cell's arithmetic reads from the state planes
+// A cell a cell pass declined, handed to the next pass: every value the cell's arithmetic reads from the state planes
 // besides the obstacle rows.  Consecutive list entries are cells of unrelated instances, so gathering them again from the
 // t-fastest planes would cost one 32-byte sector per scalar; a record is five 16-byte loads, consecutive across the warp.
 // The previous duals (dual residual) are in the record when E <= 4 and R <= 4 (rec_duals); otherwise cell_store reads them
@@ -46,8 +46,8 @@ struct rda_handle {
   int sms;               // streaming multiprocessors of the device the handle was created on
   float *lam, *mu, *z, *xi, *zeta, *dis, *coef, *pref, *cur_s, *cur_u, *ref_s, *ref_speed;
   float *resi_acc, *resi_pri, *resi_dual;
-  int *status, *iters, *done, *counters, *worklist, *worklist2;
-  // the declined cells of the polygon passes as records, two lists of B * N * T (every cell may be declined: the cold
+  int *status, *iters, *done, *counters;
+  // the declined cells of the cell passes as records, two lists of B * N * T (every cell may be declined: the cold
   // start's first iteration has no support-vertex pairs), used in turn (step_lammuz_part)
   CellRec *rec_a, *rec_b;
   char* su_ws;           // [B][su_ws_stride] global workspace of the su-QP interior point iteration (hinge slacks /
@@ -66,7 +66,7 @@ struct rda_handle {
   int launches;
   int began;
   // rda_solve runs a large batch as `parts` contiguous sub-batches on as many streams (the caller's
-  // and `side[]`), so that the latency-bound worklist passes and the tail of the su-QP kernel of one
+  // and `side[]`), so that the latency-bound listed cell passes and the tail of the su-QP kernel of one
   // sub-batch overlap the kernels of the others
   cudaStream_t side[3];
   cudaEvent_t ev_fork, ev_join[3];
@@ -106,11 +106,16 @@ struct WarpCtx {
 struct DevPtrs {
   float *lam, *mu, *z, *xi, *zeta, *dis, *coef, *pref, *cur_s, *cur_u, *ref_s, *ref_speed;
   float *resi_acc, *resi_pri, *resi_dual;
-  int *status, *iters, *done, *counters, *worklist, *worklist2;
-  int* wl_count;         // lengths of the worklists of this sub-batch ([2]: cells declined by the coherent pass)
+  int *status, *iters, *done, *counters;
+  // lengths of the record lists of this sub-batch, the same for both bodies; k_finalize clears them:
+  //   [0] first pass (k_cells_fast, k_cells_dr) -> searched pass (k_cells_mid, k_cells_dr_mid), in rec_b
+  //   [1] searched pass -> last pass (k_cells_slow_coop, k_cells_dr_slow_coop) or k_cells_extra, in rec_a
+  //   [2] coherent pass k_cells_coh -> listed first pass k_cells_fast<.., true>, in rec_a
+  //   [3] k_cells_extra -> k_cells_slow_coop, in rec_b
+  int* wl_count;
   const ObstacleGeom<4>* ogeo;
   unsigned char* feat;
-  CellRec *rec_a, *rec_b;  // record lists of the polygon cell passes (ping-pong, step_lammuz_part)
+  CellRec *rec_a, *rec_b;  // record lists of the cell passes (ping-pong, step_lammuz_part)
   char* su_ws;
   size_t su_ws_stride;
   const float *obs_A, *obs_b;
@@ -636,7 +641,7 @@ __global__ void __launch_bounds__(128) k_cells_mid(DevPtrs d, RobotGeom rb, floa
       RowsLocal rows;
       rows_preload(d, c, rows);
       CellWork<float> w;
-      cell_front<float, false>(rb, c.kind, d.E, rows.A, rows.b, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0, c.xi1, ro2, w);
+      cell_front<float>(rb, c.kind, d.E, rows.A, rows.b, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0, c.xi1, ro2, w);
       if (w.have) {
         CellOut<float> out;
         cell_back<float>(rb, w, c.zeta, theta, out);
@@ -655,11 +660,11 @@ __global__ void __launch_bounds__(128) k_cells_mid(DevPtrs d, RobotGeom rb, floa
 }
 
 // ------------------------------------------------------------------------------------------------
-// Disc body (car_tuple.cone_type 'norm2', rda_solver.py:1034-1039; cell_disc_robot.cuh).  Three passes over the
-// same worklist machinery: k_cells_dr solves every cell whose hinge is inactive in closed form (one thread per
-// cell, coalesced like the first polygon pass) and lists the rest; k_cells_dr_mid tries the searched closed forms
-// of the listed cells, one cell per thread; k_cells_dr_slow_coop runs the two-cone barrier programmes of what is
-// left, one cell per warp.
+// Disc body (car_tuple.cone_type 'norm2', rda_solver.py:1034-1039; cell_disc_robot.cuh).  Three passes that hand
+// their declined cells on as records, like the polygon passes: k_cells_dr solves every cell whose hinge is inactive in
+// closed form (one thread per cell, coalesced like the first polygon pass) and lists the rest in d.rec_b;
+// k_cells_dr_mid tries the searched closed forms of the listed cells, one cell per thread, and lists what is left in
+// d.rec_a; k_cells_dr_slow_coop runs the two-cone barrier programmes of those, one cell per warp.
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(128) k_cells_dr(DevPtrs d, RobotGeom rb, float ro2, float theta) {
   const int NT = d.N * d.T;
@@ -687,38 +692,29 @@ __global__ void __launch_bounds__(128) k_cells_dr(DevPtrs d, RobotGeom rb, float
         need = true;
       }
     }
-    const unsigned m = __ballot_sync(0xffffffffu, need);
-    if (m) {
-      int leader = __ffs(m) - 1, pos = 0;
-      if (lane == leader) pos = atomicAdd(&d.wl_count[1], __popc(m));
-      pos = __shfl_sync(0xffffffffu, pos, leader);
-      if (need) d.worklist2[pos + __popc(m & ((1u << lane) - 1))] = (int)idx;
-    }
+    if (CellRec* s = rec_slot(need, d.rec_b, &d.wl_count[0])) *s = cell_rec_load(d, idx);
     const unsigned solved = __ballot_sync(0xffffffffu, live && !need);
     if (lane == 0 && solved) atomicAdd(&d.counters[0], __popc(solved));
   }
 }
 
 // Disc body, second pass: the searched closed forms (edge and point contacts, overlap cases; point contacts in float64) for the
-// cells the first pass listed, one thread per cell; what is left (0.01 % of the cells on the bench workload) goes to the
-// cooperative barrier pass through d.worklist.
+// cells the first pass listed (records in d.rec_b), one thread per record; the records of what is left (0.01 % of the cells
+// on the bench workload) go to the cooperative barrier pass through d.rec_a.
 __global__ void __launch_bounds__(128) k_cells_dr_mid(DevPtrs d, RobotGeom rb, float ro2, float theta) {
-  const int count = d.wl_count[1];
-  const int lane = threadIdx.x & 31;
+  const int count = d.wl_count[0];
   for (int base = blockIdx.x * blockDim.x; base < count; base += gridDim.x * blockDim.x) {
     const int wi = base + threadIdx.x;
     bool need = false;
-    int idx = 0;
     if (wi < count) {
-      idx = d.worklist2[wi];
-      CellIn c = cell_load(d, idx);
+      CellIn c = cell_from_rec(d, d.rec_b[wi]);
       CellWork<float> w;
       cell_front_dr<float>(rb, c.kind, d.E, c.A, c.bb, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0, c.xi1, ro2, w, true);
       if (w.have) {
         CellOut<float> out;
         cell_back_dr<float>(rb, w, c.zeta, theta, out);
         float hm2 = 0.f, dual = 0.f;
-        cell_store(d, c, out, &hm2, &dual);
+        cell_store(d, c, out, &hm2, &dual, d.rec_b + wi);
         atomicAdd(&d.resi_acc[2 * c.b], hm2);
         atomicAdd(&d.resi_acc[2 * c.b + 1], dual);
         atomicAdd(&d.counters[0], 1);
@@ -726,13 +722,7 @@ __global__ void __launch_bounds__(128) k_cells_dr_mid(DevPtrs d, RobotGeom rb, f
         need = true;
       }
     }
-    const unsigned m = __ballot_sync(0xffffffffu, need);
-    if (m) {
-      int leader = __ffs(m) - 1, pos = 0;
-      if (lane == leader) pos = atomicAdd(&d.wl_count[4], __popc(m));
-      pos = __shfl_sync(0xffffffffu, pos, leader);
-      if (need) d.worklist[pos + __popc(m & ((1u << lane) - 1))] = idx;
-    }
+    if (CellRec* s = rec_slot(need, d.rec_a, &d.wl_count[1])) *s = d.rec_b[wi];
   }
 }
 
@@ -742,17 +732,16 @@ constexpr int COOP_WARPS = 4;
 // one cell per WARP: the two-cone barrier iterations spread over the lanes, the problem in shared memory
 __global__ void __launch_bounds__(32 * COOP_WARPS) k_cells_dr_slow_coop(DevPtrs d, RobotGeom rb, float ro2, float theta) {
   __shared__ DiscSlowStore store[COOP_WARPS];
-  const int count = d.wl_count[4];          // what k_cells_dr_mid left, in d.worklist
+  const int count = d.wl_count[1];          // what k_cells_dr_mid left, in d.rec_a
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   DiscSlowStore& S = store[warp];
   WarpCtx ctx;
   for (int wi = blockIdx.x * COOP_WARPS + warp; wi < count; wi += gridDim.x * COOP_WARPS) {
-    const long long idx = d.worklist[wi];
     CellIn c;
     CellWork<float> w;
     w.have = false;
     if (lane == 0) {
-      c = cell_load(d, idx);
+      c = cell_from_rec(d, d.rec_a[wi]);
       // geometry only: the closed forms have been tried by k_cells_dr_mid
       cell_front_dr<float>(rb, c.kind, d.E, c.A, c.bb, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0, c.xi1, ro2, w, false);
     }
@@ -771,6 +760,8 @@ __global__ void __launch_bounds__(32 * COOP_WARPS) k_cells_dr_slow_coop(DevPtrs 
         dual = INFINITY;
         atomicOr(&d.status[c.b], RDA_ST_CELL_FALLBACK);
       } else {
+        // previous duals from the planes (the same values): read from the record, they stay live across the barrier
+        // solve's calls and add 48 bytes of spills to this lane
         cell_store(d, c, out, &hm2, &dual);
       }
       atomicAdd(&d.resi_acc[2 * c.b], hm2);
@@ -796,7 +787,7 @@ __global__ void __launch_bounds__(128) k_cells_extra(DevPtrs d, RobotGeom rb, fl
       RowsLocal rows;
       rows_preload(d, c, rows);
       CellWork<float> w;
-      cell_front<float, false, true>(rb, c.kind, d.E, rows.A, rows.b, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0, c.xi1, ro2, w);
+      cell_front<float, true>(rb, c.kind, d.E, rows.A, rows.b, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0, c.xi1, ro2, w);
       if (w.have) {
         CellOut<float> out;
         cell_back<float>(rb, w, c.zeta, theta, out);
@@ -809,7 +800,7 @@ __global__ void __launch_bounds__(128) k_cells_extra(DevPtrs d, RobotGeom rb, fl
         need = true;
       }
     }
-    if (CellRec* s = rec_slot(need, d.rec_b, &d.wl_count[4])) *s = d.rec_a[wi];
+    if (CellRec* s = rec_slot(need, d.rec_b, &d.wl_count[3])) *s = d.rec_a[wi];
   }
 }
 
@@ -821,7 +812,7 @@ __global__ void __launch_bounds__(32 * COOP_WARPS) k_cells_slow_coop(DevPtrs d, 
   __shared__ CellSlowStore store[COOP_WARPS];
   // from_extra: the records k_cells_extra left — d.rec_b (the first pass' list, consumed by now) with its own counter;
   // otherwise the searched pass' own leftovers in d.rec_a (small batches: one launch less, lane 0 runs the EXTRA closed forms)
-  const int count = from_extra ? d.wl_count[4] : d.wl_count[1];
+  const int count = from_extra ? d.wl_count[3] : d.wl_count[1];
   const CellRec* list = from_extra ? d.rec_b : d.rec_a;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   CellSlowStore& S = store[warp];
@@ -832,7 +823,7 @@ __global__ void __launch_bounds__(32 * COOP_WARPS) k_cells_slow_coop(DevPtrs d, 
     w.have = false;
     if (lane == 0) {
       c = cell_from_rec(d, list[wi]);
-      cell_front<float, false, true>(rb, c.kind, d.E, c.A, c.bb, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0, c.xi1, ro2, w);
+      cell_front<float, true>(rb, c.kind, d.E, c.A, c.bb, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0, c.xi1, ro2, w);
     }
     const int have = __shfl_sync(0xffffffffu, (int)w.have, 0);
     if (!have) {
@@ -885,7 +876,7 @@ __device__ __forceinline__ void finalize_instance(const DevPtrs& d, const RobotG
 
 __global__ void k_finalize(DevPtrs d, RobotGeom rb, float thr) {
   int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b == 0) { d.wl_count[0] = 0; d.wl_count[1] = 0; d.wl_count[2] = 0; d.wl_count[3] = 0; d.wl_count[4] = 0; }   // worklists consumed
+  if (b == 0) { d.wl_count[0] = 0; d.wl_count[1] = 0; d.wl_count[2] = 0; d.wl_count[3] = 0; }   // record lists consumed
   if (b >= d.B) return;
   if (d.done[b]) return;
   finalize_instance(d, rb, thr, b);
@@ -1021,7 +1012,7 @@ __global__ void __launch_bounds__(128, 2) k_admm_small(DevPtrs d, SuParams P, Ro
       for (int idx = tid; idx < NT; idx += nth) {
         CellIn c = cell_load(ds, idx);
         CellWork<float> w;
-        cell_front<float, false, true>(rb, c.kind, E, c.A, c.bb, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0, c.xi1, ro2, w);
+        cell_front<float, true>(rb, c.kind, E, c.A, c.bb, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0, c.xi1, ro2, w);
         wl[1 + idx] = !w.have;
         if (!w.have) continue;
         CellOut<float> o;
@@ -1048,7 +1039,7 @@ __global__ void __launch_bounds__(128, 2) k_admm_small(DevPtrs d, SuParams P, Ro
           w.have = false;
           if (lane == 0) {
             c = cell_load(ds, idx);
-            cell_front<float, false, true>(rb, c.kind, E, c.A, c.bb, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0, c.xi1, ro2, w);
+            cell_front<float, true>(rb, c.kind, E, c.A, c.bb, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0, c.xi1, ro2, w);
           }
           __syncwarp();
           cell_slow<float, WarpCtx>(rb, w, S, ctx);
@@ -1158,7 +1149,7 @@ __global__ void k_fill(float* p, float v, size_t n) {
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) p[i] = v;
 }
 
-// pointers of the sub-batch [b0, b0 + nb) (part = 0, 1 selects its worklist counters)
+// pointers of the sub-batch [b0, b0 + nb) (part selects its list counters)
 DevPtrs dev_ptrs(const rda_handle* h, int b0, int nb, int part) {
   DevPtrs d;
   const size_t o = (size_t)b0, T = h->T, N = h->N, E = h->E, R = h->R, NT = N * T;
@@ -1172,9 +1163,7 @@ DevPtrs dev_ptrs(const rda_handle* h, int b0, int nb, int part) {
   d.counters = h->counters; d.wl_count = h->counters + 8 + 8 * part;     // part < 4, 8 counters each
   d.ogeo = h->ogeo ? h->ogeo + o * N : nullptr;
   d.feat = h->feat ? h->feat + o * NT : nullptr;
-  d.rec_a = h->rec_a ? h->rec_a + o * NT : nullptr;
-  d.rec_b = h->rec_b ? h->rec_b + o * NT : nullptr;
-  d.worklist = h->worklist + o * NT; d.worklist2 = h->worklist2 + o * NT;
+  d.rec_a = h->rec_a + o * NT; d.rec_b = h->rec_b + o * NT;
   d.su_ws = h->su_ws + o * h->su_ws_stride; d.su_ws_stride = h->su_ws_stride;
   d.obs_A = h->obs_A ? h->obs_A + o * N * Tc * E * 2 : nullptr;
   d.obs_b = h->obs_b ? h->obs_b + o * N * Tc * E : nullptr;
@@ -1248,13 +1237,9 @@ int rda_create(const rda_config* cfg, const rda_tunables* tun, rda_handle** out)
   alloc(&h->cur_u, B * 2 * T); alloc(&h->ref_s, B * 3 * (T + 1)); alloc(&h->ref_speed, B);
   alloc(&h->resi_acc, B * 2); alloc(&h->resi_pri, B); alloc(&h->resi_dual, B);
   alloc((float**)&h->status, B); alloc((float**)&h->iters, B); alloc((float**)&h->done, B);
-  alloc((float**)&h->counters, 64);     // [0..7] statistics, [8 + 8 part ..] worklist lengths of the sub-batches
-  alloc((float**)&h->worklist, B * NT);
-  alloc((float**)&h->worklist2, B * NT);
-  if (!h->rb.disc) {     // the disc body's passes list cell indices (worklist, worklist2)
-    alloc((float**)&h->rec_a, B * NT * (sizeof(CellRec) / 4));
-    alloc((float**)&h->rec_b, B * NT * (sizeof(CellRec) / 4));
-  }
+  alloc((float**)&h->counters, 64);     // [0..7] statistics, [8 + 8 part ..] record list lengths of the sub-batches
+  alloc((float**)&h->rec_a, B * NT * (sizeof(CellRec) / 4));
+  alloc((float**)&h->rec_b, B * NT * (sizeof(CellRec) / 4));
   alloc((float**)&h->su_ws, B * (h->su_ws_stride / 4));
   if (e != cudaSuccess) { rda_destroy(h); return (int)e; }
   e = cfg->su_fp64 ? cudaFuncSetAttribute(k_su<double>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)
@@ -1314,7 +1299,7 @@ int rda_destroy(rda_handle* h) {
   if (!h) return RDA_E_ARG;
   float* bufs[] = {h->lam, h->mu, h->z, h->xi, h->zeta, h->dis, h->coef, h->pref, h->cur_s, h->cur_u,
                    h->ref_s, h->ref_speed, h->resi_acc, h->resi_pri, h->resi_dual, (float*)h->status,
-                   (float*)h->iters, (float*)h->done, (float*)h->counters, (float*)h->worklist, (float*)h->worklist2, (float*)h->su_ws};
+                   (float*)h->iters, (float*)h->done, (float*)h->counters, (float*)h->su_ws};
   for (float* p : bufs) if (p) cudaFree(p);
   if (h->ogeo) cudaFree(h->ogeo);
   if (h->feat) cudaFree(h->feat);
@@ -1379,7 +1364,7 @@ int rda_reset(rda_handle* h, void* stream) {
   return 0;
 }
 
-// ---- the launches of one sub-batch [b0, b0 + nb) on stream s (part selects its worklist counters) ----
+// ---- the launches of one sub-batch [b0, b0 + nb) on stream s (part selects its list counters) ----
 static int begin_part(rda_handle* h, const rda_inputs* in, int b0, int nb, int part, cudaStream_t s) {
   DevPtrs d = dev_ptrs(h, b0, nb, part);
   const size_t o = (size_t)b0, T = h->T;
