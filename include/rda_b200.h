@@ -186,6 +186,34 @@ int rda_convert_world_obstacles(int B, int W, int N, int T, int E, float dt, int
                                 const float *shape_radius, const float *shape_vel, float *obs_A,
                                 float *obs_b, int32_t *obs_kind, int32_t *obs_count, void *cuda_stream);
 
+/* A FLEET that avoids itself: robots that share a world see each other as moving obstacles, as each reference MPC
+ * receives the other agents from its simulator (the dynamic_obs example: obs(center, radius, vertex, cone_type,
+ * velocity), predicted at constant velocity, mpc.py:440-474).
+ * rda_fleet_shapes writes every robot as one raw shape (layout of rda_convert_world_obstacles, [B] entries): the
+ * robot body (RDA_OBS_POLYGON: body_nv counter-clockwise vertices body_xy [body_nv][2] in the body frame, 3..8;
+ * RDA_OBS_CIRCLE: centre body_xy[0..1], body_radius > 0) placed at the pose state [B][3] (p + R(theta) v), with the
+ * world-frame velocity of the first control of cur_vel [B][2][T], the one rda_motion_predict moved the robot with:
+ * v (cos theta, sin theta) for acker / diff, v (cos psi, sin psi) for omni (mpc.py:293-336).
+ * rda_convert_fleet_obstacles is rda_convert_world_obstacles over a longer list per robot: every shape of its world
+ * in world order, then every other robot of the same world in ascending robot index, whose shapes are entry m of
+ * fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel (rda_fleet_shapes' outputs).  The robots of world w are
+ * fleet_robot [fleet_start[w], fleet_start[w+1]) (fleet_start [W+1], fleet_robot [B]), in ascending order, and must
+ * be exactly the robots whose robot_world is w: a stable sort of robot_world and a search for 0..W give both.
+ * Sort key, stable order, the first N, padding, rows and time_varying layout are those of rda_convert_world_obstacles;
+ * obs_count [B] receives the world size plus the robots of the world minus one.  A robot whose robot_world is outside
+ * [0, W) neither sees nor is seen.  rda_convert_world_obstacles is this call without the fleet.                */
+int rda_fleet_shapes(int B, int T, int dynamics, int body_kind, int body_nv, const float *body_xy,
+                     float body_radius, const float *state, const float *cur_vel, int32_t *shape_kind,
+                     int32_t *shape_nv, float *shape_xy, float *shape_radius, float *shape_vel, void *cuda_stream);
+int rda_convert_fleet_obstacles(int B, int W, int N, int T, int E, float dt, int time_varying, int order,
+                                const float *state, const int32_t *world_start, const int32_t *robot_world,
+                                const int32_t *shape_kind, const int32_t *shape_nv, const float *shape_xy,
+                                const float *shape_radius, const float *shape_vel, const int32_t *fleet_start,
+                                const int32_t *fleet_robot, const int32_t *fleet_kind, const int32_t *fleet_nv,
+                                const float *fleet_xy, const float *fleet_radius, const float *fleet_vel,
+                                float *obs_A, float *obs_b, int32_t *obs_kind, int32_t *obs_count,
+                                void *cuda_stream);
+
 /* Arrive rule of MPC.control (mpc.py:170-185, single gear): instances whose near_index >=
  * P - goal_index_threshold get u_opt = 0 and arrive = 1; cur_vel (may be NULL) receives the
  * controls kept as the next step's nominal (mpc.py:186).  u_opt, cur_vel [B][2][T].        */

@@ -48,7 +48,7 @@ EXPORTS = ['rda_create', 'rda_destroy', 'rda_set_tunables', 'rda_get_tunables', 
            'rda_get_buffer', 'rda_copy_buffer', 'rda_last_launch_count', 'rda_version',
            'rda_pre_process', 'rda_convert_obstacles', 'rda_post_process', 'rda_motion_predict',
            'rda_pre_process_curves', 'rda_post_process_gear', 'rda_convert_world_obstacles',
-           'rda_pre_process_paths', 'rda_post_process_paths']
+           'rda_pre_process_paths', 'rda_post_process_paths', 'rda_fleet_shapes', 'rda_convert_fleet_obstacles']
 MAX_SHAPES = 64
 MAX_WORLD_SLOTS = 256
 
@@ -93,6 +93,8 @@ def load():
                                           vp]
     lib.rda_post_process_paths.argtypes = [i, i, i, vp, vp, vp, i, vp, vp, vp, vp, vp, vp]
     lib.rda_motion_predict.argtypes = [i, i, i, f, f, vp, vp, vp]
+    lib.rda_fleet_shapes.argtypes = [i, i, i, i, i, vp, f] + [vp] * 8
+    lib.rda_convert_fleet_obstacles.argtypes = [i, i, i, i, i, f, i, i] + [vp] * 20
     for name in EXPORTS:
         if name != 'rda_version':
             getattr(lib, name).restype = C.c_int

@@ -232,6 +232,34 @@ RDA_HD void obstacle_rows(int kind, int nv, const float* xy, double radius, doub
   }
 }
 
+// A robot of a fleet as one raw shape for its map-mates: the body (body frame: polygon vertices body_xy [nv][2],
+// counter-clockwise, or the disc centre body_xy[0..1] and body_radius) placed at the pose `state` (p + R(theta) v),
+// moving with the world-frame velocity of its control (v0, v1) as motion_predict moves it: v0 (cos, sin) of the
+// heading for acker / diff, of the control angle v1 for omni (mpc.py:293-336).  Entries of xy beyond the shape's own
+// are zero, as the host packing leaves them.
+RDA_HD void fleet_shape(int dynamics, int body_kind, int body_nv, const float* body_xy, float body_radius,
+                        const float* state, double v0, double v1, int* kind, int* nv, float* xy, float* radius,
+                        float* vel) {
+  const double px = state[0], py = state[1], th = state[2];
+  const double c = cos(th), s = sin(th);
+  const int n = body_kind == RDA_OBS_CIRCLE ? 1 : body_nv;
+  for (int i = 0; i < RDA_MAX_EDGE; ++i) {
+    if (i < n) {
+      const double bx = body_xy[2 * i], by = body_xy[2 * i + 1];
+      xy[2 * i] = (float)(px + (c * bx - s * by));
+      xy[2 * i + 1] = (float)(py + (s * bx + c * by));
+    } else {
+      xy[2 * i] = 0.f; xy[2 * i + 1] = 0.f;
+    }
+  }
+  *kind = body_kind;
+  *nv = body_kind == RDA_OBS_CIRCLE ? 0 : body_nv;
+  *radius = body_kind == RDA_OBS_CIRCLE ? body_radius : 0.f;
+  const double dir = dynamics == RDA_DYN_OMNI ? v1 : th;
+  vel[0] = (float)(v0 * cos(dir));
+  vel[1] = (float)(v0 * sin(dir));
+}
+
 // the order of the stable sort by key: ties go to the lower list index
 RDA_HD bool obstacle_before(double ka, int ia, double kb, int ib) { return ka < kb || (ka == kb && ia < ib); }
 

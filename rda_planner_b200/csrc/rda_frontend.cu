@@ -108,10 +108,29 @@ __device__ __forceinline__ int world_rank(const double* key, const int* idx, int
   return lo;
 }
 
+// The raw shapes a robot chooses from: its world's shapes [first, first + n_world), then, with a fleet, its map-mates:
+// the robots of fleet_robot [mate0, mate0 + mates + 1) other than the robot itself, whose shapes are entry m of the
+// fleet arrays.  Each world's robots are listed in ascending order, so skipping the robot is one comparison.
+struct ShapeList {
+  int first, n_world, mate0, mates;
+};
+
+__device__ __forceinline__ size_t list_entry(const ShapeList& L, int i, const int* fleet_robot, int b, int B,
+                                             bool* mate) {
+  *mate = i >= L.n_world;
+  if (!*mate) return (size_t)L.first + i;
+  const int p = L.mate0 + (i - L.n_world);
+  int m = fleet_robot[p];
+  if (m >= b) m = fleet_robot[p + 1];
+  return (size_t)(m < 0 ? 0 : (m >= B ? B - 1 : m));   // a malformed list never reads outside the fleet
+}
+
 __global__ void __launch_bounds__(kWorldTile)
 k_convert_world_obstacles(int B, int W, int N, int T, int E, float dt, int time_varying, int order, const float* state,
                           const int* world_start, const int* robot_world, const int* shape_kind, const int* shape_nv,
-                          const float* shape_xy, const float* shape_radius, const float* shape_vel, float* obs_A,
+                          const float* shape_xy, const float* shape_radius, const float* shape_vel,
+                          const int* fleet_start, const int* fleet_robot, const int* fleet_kind, const int* fleet_nv,
+                          const float* fleet_xy, const float* fleet_radius, const float* fleet_vel, float* obs_A,
                           float* obs_b, int* obs_kind, int* obs_count) {
   // dynamic shared memory (order != 0): kept keys [2][N], candidate keys [2][tile], kept indices [2][N],
   // candidate indices [2][tile]; the kept list is double-buffered, candidates are gathered then sorted
@@ -121,12 +140,18 @@ k_convert_world_obstacles(int B, int W, int N, int T, int E, float dt, int time_
   if (b >= B) return;
   const int tid = threadIdx.x;
   const int w = robot_world ? robot_world[b] : 0;
-  int first = 0, count = 0;
+  ShapeList L = {0, 0, 0, 0};
   if (w >= 0 && w < W) {
-    first = world_start[w];
-    count = world_start[w + 1] - first;
-    if (count < 0) count = 0;
+    L.first = world_start[w];
+    L.n_world = world_start[w + 1] - L.first;
+    if (L.n_world < 0) L.n_world = 0;
+    if (fleet_start) {                                 // NULL: no fleet, the world's shapes only
+      L.mate0 = fleet_start[w];
+      L.mates = fleet_start[w + 1] - L.mate0 - 1;
+      if (L.mates < 0) L.mates = 0;
+    }
   }
+  const int count = L.n_world + L.mates;               // positions in the list: world shapes, then map-mates
   int cur = 0;
   int* kept_idx = nullptr;
   if (order && count > 0) {
@@ -143,8 +168,10 @@ k_convert_world_obstacles(int B, int W, int N, int T, int E, float dt, int time_
     for (int base = 0, tile = 0; base < count; base += kWorldTile, tile = tile == 2 ? 0 : tile + 1) {
       const int i = base + tid;
       if (i < count) {
-        const size_t s = (size_t)first + i;
-        const double key = obstacle_key(shape_kind[s], shape_nv[s], shape_xy + s * RDA_MAX_EDGE * 2, sx, sy);
+        bool mate;
+        const size_t s = list_entry(L, i, fleet_robot, b, B, &mate);
+        const double key = obstacle_key((mate ? fleet_kind : shape_kind)[s], (mate ? fleet_nv : shape_nv)[s],
+                                        (mate ? fleet_xy : shape_xy) + s * RDA_MAX_EDGE * 2, sx, sy);
         if (nk < N || key < kkey[cur * N + N - 1]) {
           const int p = atomicAdd(&n_cand[tile], 1);
           ckey[p] = key; cidx[p] = i;
@@ -194,13 +221,28 @@ k_convert_world_obstacles(int B, int W, int N, int T, int E, float dt, int time_
     }
     const int slot = n < count ? n : count - 1;        // pad by repeating the last
     int src = kept_idx ? kept_idx[slot] : slot;
-    if (src < 0 || src >= count) src = count - 1;      // NaN keys have no order; never read outside the world
-    const size_t s = (size_t)first + src;
-    const int kind = shape_kind[s];
+    if (src < 0 || src >= count) src = count - 1;      // NaN keys have no order; never read outside the list
+    bool mate;
+    const size_t s = list_entry(L, src, fleet_robot, b, B, &mate);
+    const int kind = (mate ? fleet_kind : shape_kind)[s];
     if (t == 0) obs_kind[(size_t)b * N + n] = kind;
-    obstacle_rows(kind, shape_nv[s], shape_xy + s * RDA_MAX_EDGE * 2, shape_radius[s], shape_vel[2 * s],
-                  shape_vel[2 * s + 1], t, (double)dt, E, A, bb);
+    const float* vel = (mate ? fleet_vel : shape_vel) + 2 * s;
+    obstacle_rows(kind, (mate ? fleet_nv : shape_nv)[s], (mate ? fleet_xy : shape_xy) + s * RDA_MAX_EDGE * 2,
+                  (mate ? fleet_radius : shape_radius)[s], vel[0], vel[1], t, (double)dt, E, A, bb);
   }
+}
+
+// Each robot of a fleet as a raw shape for its map-mates (fleet_shape), one thread per robot: its body at its pose,
+// moving with the first control of cur_vel, the one rda_motion_predict moved it with.
+__global__ void k_fleet_shapes(int B, int T, int dynamics, int body_kind, int body_nv, const float* body_xy,
+                               float body_radius, const float* state, const float* cur_vel, int* shape_kind,
+                               int* shape_nv, float* shape_xy, float* shape_radius, float* shape_vel) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const float* u = cur_vel + (size_t)b * 2 * T;
+  fleet_shape(dynamics, body_kind, body_nv, body_xy, body_radius, state + 3 * (size_t)b, (double)u[0], (double)u[T],
+              shape_kind + b, shape_nv + b, shape_xy + (size_t)b * RDA_MAX_EDGE * 2, shape_radius + b,
+              shape_vel + 2 * (size_t)b);
 }
 
 // End-of-curve and arrive rules of MPC.control (mpc.py:166-185) on each robot's own curve and path, one thread per
@@ -239,6 +281,30 @@ __global__ void k_motion_predict(int B, int T, int dynamics, float dt, float L, 
   double o[3];
   motion_predict(dynamics, (double)dt, (double)L, s, (double)u_opt[(size_t)b * 2 * T], (double)u_opt[(size_t)b * 2 * T + T], o);
   state[3 * b] = (float)o[0]; state[3 * b + 1] = (float)o[1]; state[3 * b + 2] = (float)o[2];
+}
+
+// Argument checks and launch of k_convert_world_obstacles.  Without `fleet` the fleet pointers are NULL and each robot
+// chooses from its world's shapes only.
+int launch_world_obstacles(bool fleet, int B, int W, int N, int T, int E, float dt, int time_varying, int order,
+                           const float* state, const int32_t* world_start, const int32_t* robot_world,
+                           const int32_t* shape_kind, const int32_t* shape_nv, const float* shape_xy,
+                           const float* shape_radius, const float* shape_vel, const int32_t* fleet_start,
+                           const int32_t* fleet_robot, const int32_t* fleet_kind, const int32_t* fleet_nv,
+                           const float* fleet_xy, const float* fleet_radius, const float* fleet_vel, float* obs_A,
+                           float* obs_b, int32_t* obs_kind, int32_t* obs_count, cudaStream_t stream) {
+  if (B < 1 || W < 1 || N < 1 || T < 1) return RDA_E_ARG;
+  if (N > RDA_MAX_WORLD_SLOTS || E < 3 || E > RDA_MAX_EDGE) return RDA_E_UNSUPPORTED;
+  if (!world_start || !shape_kind || !shape_nv || !shape_xy || !shape_radius || !shape_vel) return RDA_E_ARG;
+  if (!obs_A || !obs_b || !obs_kind || !obs_count || (order && !state)) return RDA_E_ARG;
+  if (fleet && (!fleet_start || !fleet_robot || !fleet_kind || !fleet_nv || !fleet_xy || !fleet_radius || !fleet_vel))
+    return RDA_E_ARG;
+  const size_t smem = order ? (size_t)(2 * N + 2 * kWorldTile) * (sizeof(double) + sizeof(int)) : 0;
+  k_convert_world_obstacles<<<B, kWorldTile, smem, stream>>>(
+      B, W, N, T, E, dt, time_varying, order, state, world_start, robot_world, shape_kind, shape_nv, shape_xy,
+      shape_radius, shape_vel, fleet_start, fleet_robot, fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel,
+      obs_A, obs_b, obs_kind, obs_count);
+  RDA_CUDA(cudaGetLastError());
+  return 0;
 }
 
 }  // namespace
@@ -327,16 +393,41 @@ int rda_convert_world_obstacles(int B, int W, int N, int T, int E, float dt, int
                                 const int32_t* shape_kind, const int32_t* shape_nv, const float* shape_xy,
                                 const float* shape_radius, const float* shape_vel, float* obs_A, float* obs_b,
                                 int32_t* obs_kind, int32_t* obs_count, void* stream) {
-  if (B < 1 || W < 1 || N < 1 || T < 1) return RDA_E_ARG;
-  if (N > RDA_MAX_WORLD_SLOTS || E < 3 || E > RDA_MAX_EDGE) return RDA_E_UNSUPPORTED;
-  if (!world_start || !shape_kind || !shape_nv || !shape_xy || !shape_radius || !shape_vel) return RDA_E_ARG;
-  if (!obs_A || !obs_b || !obs_kind || !obs_count || (order && !state)) return RDA_E_ARG;
-  const size_t smem = order ? (size_t)(2 * N + 2 * kWorldTile) * (sizeof(double) + sizeof(int)) : 0;
-  k_convert_world_obstacles<<<B, kWorldTile, smem, (cudaStream_t)stream>>>(
-      B, W, N, T, E, dt, time_varying, order, state, world_start, robot_world, shape_kind, shape_nv, shape_xy,
-      shape_radius, shape_vel, obs_A, obs_b, obs_kind, obs_count);
+  return launch_world_obstacles(false, B, W, N, T, E, dt, time_varying, order, state, world_start, robot_world,
+                                shape_kind, shape_nv, shape_xy, shape_radius, shape_vel, nullptr, nullptr, nullptr,
+                                nullptr, nullptr, nullptr, nullptr, obs_A, obs_b, obs_kind, obs_count,
+                                (cudaStream_t)stream);
+}
+
+int rda_fleet_shapes(int B, int T, int dynamics, int body_kind, int body_nv, const float* body_xy, float body_radius,
+                     const float* state, const float* cur_vel, int32_t* shape_kind, int32_t* shape_nv, float* shape_xy,
+                     float* shape_radius, float* shape_vel, void* stream) {
+  if (B < 1 || T < 1 || dynamics < 0 || dynamics > 2) return RDA_E_ARG;
+  if (body_kind == RDA_OBS_POLYGON) {
+    if (body_nv < 3 || body_nv > RDA_MAX_EDGE) return RDA_E_UNSUPPORTED;
+  } else if (body_kind != RDA_OBS_CIRCLE || !(body_radius > 0.f)) {
+    return RDA_E_ARG;
+  }
+  if (!body_xy || !state || !cur_vel || !shape_kind || !shape_nv || !shape_xy || !shape_radius || !shape_vel)
+    return RDA_E_ARG;
+  k_fleet_shapes<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(B, T, dynamics, body_kind, body_nv, body_xy,
+                                                                     body_radius, state, cur_vel, shape_kind, shape_nv,
+                                                                     shape_xy, shape_radius, shape_vel);
   RDA_CUDA(cudaGetLastError());
   return 0;
+}
+
+int rda_convert_fleet_obstacles(int B, int W, int N, int T, int E, float dt, int time_varying, int order,
+                                const float* state, const int32_t* world_start, const int32_t* robot_world,
+                                const int32_t* shape_kind, const int32_t* shape_nv, const float* shape_xy,
+                                const float* shape_radius, const float* shape_vel, const int32_t* fleet_start,
+                                const int32_t* fleet_robot, const int32_t* fleet_kind, const int32_t* fleet_nv,
+                                const float* fleet_xy, const float* fleet_radius, const float* fleet_vel, float* obs_A,
+                                float* obs_b, int32_t* obs_kind, int32_t* obs_count, void* stream) {
+  return launch_world_obstacles(true, B, W, N, T, E, dt, time_varying, order, state, world_start, robot_world,
+                                shape_kind, shape_nv, shape_xy, shape_radius, shape_vel, fleet_start, fleet_robot,
+                                fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel, obs_A, obs_b, obs_kind,
+                                obs_count, (cudaStream_t)stream);
 }
 
 int rda_post_process(int B, int T, int P, int goal_index_threshold, const int32_t* near_index, float* u_opt,

@@ -6,6 +6,8 @@
   convert_world_obstacles_batch
                            the same over obstacle worlds of any size shared by many robots: each
                            robot's N nearest shapes of its world
+  fleet_shapes_batch, convert_fleet_obstacles_batch
+                           the same with the other robots of each world as moving obstacles
   pack_paths               a set of reference paths cut into single-gear curves (split_path, mpc.py:232-249),
                            in the layout the device reads
   BatchedMPC               MPC.control for B robots, on one reference path or each on its own path of a
@@ -18,7 +20,7 @@ import numpy as np
 import torch
 
 from . import _cabi
-from .rda_solver import RDA_solver
+from .rda_solver import RDA_solver, canonical_polygon_rows
 
 
 def _ptr(t):
@@ -209,6 +211,81 @@ def convert_world_obstacles_batch(world, state, robot_world, N, T, E, dt, time_v
     return A, b, kind, count
 
 
+def robot_body(car_tuple):
+    """The robot body of car_tuple in its own frame, as one raw shape for the other robots of a fleet: dict kind
+    (OBS_POLYGON / OBS_CIRCLE), nv, xy [8,2] float32, radius.  A polygon body is given by the vertices of its canonical
+    rows (canonical_polygon_rows, the rows the solver holds), counter-clockwise, vertex i joining rows i-1 and i,
+    computed in float64 and rounded to float32; a disc body by its centre (h0, h1) in xy[0] and its radius -h2."""
+    G = np.asarray(car_tuple.G, float)
+    h = np.asarray(car_tuple.h, float).reshape(-1)
+    xy = np.zeros((_cabi.MAX_EDGE, 2), np.float32)
+    if car_tuple.cone_type == 'norm2':
+        xy[0] = h[:2]
+        return {'kind': _cabi.OBS_CIRCLE, 'nv': 0, 'xy': xy, 'radius': float(np.float32(-h[2]))}
+    G, h = canonical_polygon_rows(G, h)
+    Gp, hp = np.roll(G, 1, axis=0), np.roll(h, 1)
+    det = Gp[:, 0] * G[:, 1] - Gp[:, 1] * G[:, 0]
+    V = np.stack([(hp * G[:, 1] - h * Gp[:, 1]) / det, (Gp[:, 0] * h - G[:, 0] * hp) / det], axis=1)
+    xy[:len(V)] = V
+    return {'kind': _cabi.OBS_POLYGON, 'nv': len(V), 'xy': xy, 'radius': 0.0}
+
+
+def fleet_shapes_batch(state, cur_vel, body, dynamics):
+    """CUDA tensors state [B,3], cur_vel [B,2,T] (the controls each robot last applied in cur_vel[:, :, 0]); body from
+    robot_body with xy a CUDA tensor.  Returns every robot as one raw shape for its map-mates, dict of CUDA tensors in
+    the layout of pack_worlds without 'start': its body at its pose, moving with the world-frame velocity of its
+    control."""
+    lib = _cabi.load()
+    dev = state.device
+    B, T = state.shape[0], cur_vel.shape[2]
+    out = {'kind': torch.empty(B, dtype=torch.int32, device=dev), 'nv': torch.empty(B, dtype=torch.int32, device=dev),
+           'xy': torch.empty((B, _cabi.MAX_EDGE, 2), dtype=torch.float32, device=dev),
+           'radius': torch.empty(B, dtype=torch.float32, device=dev),
+           'vel': torch.empty((B, 2), dtype=torch.float32, device=dev)}
+    with torch.cuda.device(dev):
+        _cabi.check(lib.rda_fleet_shapes(B, T, _cabi.DYNAMICS[dynamics], body['kind'], body['nv'], _ptr(body['xy']),
+                                         body['radius'], _ptr(state), _ptr(cur_vel), _ptr(out['kind']), _ptr(out['nv']),
+                                         _ptr(out['xy']), _ptr(out['radius']), _ptr(out['vel']), _stream(dev)),
+                    'rda_fleet_shapes')
+    return out
+
+
+def fleet_csr(robot_world, W):
+    """robot_world [B] int32 CUDA tensor -> (start [W+1], robots [B]) int32: the robots of world w are
+    robots[start[w]:start[w+1]], in ascending order; robots outside [0, W) are in no world.  On the device, without a
+    host synchronisation."""
+    ordered, robots = torch.sort(robot_world, stable=True)
+    bounds = torch.arange(W + 1, dtype=ordered.dtype, device=ordered.device)
+    start = torch.searchsorted(ordered, bounds, out_int32=True)
+    return start, robots.to(torch.int32)
+
+
+def convert_fleet_obstacles_batch(world, state, robot_world, fleet, N, T, E, dt, time_varying=False, order=True):
+    """convert_world_obstacles_batch with the robots as obstacles of each other: robot b chooses from every shape of
+    its world followed by every other robot of its world in ascending index, fleet [m] being robot m's shape (from
+    fleet_shapes_batch).  robot_world [B] int32 or None (every robot in world 0).  Returns obs_A [B,N,Tc,E,2], obs_b [B,N,Tc,E], obs_kind [B,N], obs_count [B] (world
+    size plus the robots of the world minus one)."""
+    lib = _cabi.load()
+    dev = state.device
+    B, W = state.shape[0], world['start'].shape[0] - 1
+    csr = fleet_csr(robot_world if robot_world is not None else torch.zeros(B, dtype=torch.int32, device=dev), W)
+    Tc = T + 1 if time_varying else 1
+    A = torch.empty((B, N, Tc, E, 2), dtype=torch.float32, device=dev)
+    b = torch.empty((B, N, Tc, E), dtype=torch.float32, device=dev)
+    kind = torch.empty((B, N), dtype=torch.int32, device=dev)
+    count = torch.empty(B, dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        _cabi.check(lib.rda_convert_fleet_obstacles(B, W, N, T, E, dt, int(time_varying), int(order), _ptr(state),
+                                                    _ptr(world['start']), _ptr(robot_world), _ptr(world['kind']),
+                                                    _ptr(world['nv']), _ptr(world['xy']), _ptr(world['radius']),
+                                                    _ptr(world['vel']), _ptr(csr[0]), _ptr(csr[1]), _ptr(fleet['kind']),
+                                                    _ptr(fleet['nv']), _ptr(fleet['xy']), _ptr(fleet['radius']),
+                                                    _ptr(fleet['vel']), _ptr(A), _ptr(b), _ptr(kind), _ptr(count),
+                                                    _stream(dev)),
+                    'rda_convert_fleet_obstacles')
+    return A, b, kind, count
+
+
 def shapes_to_device(shapes, device):
     return {k: torch.as_tensor(v, device=device).contiguous() for k, v in shapes.items()}
 
@@ -223,7 +300,11 @@ class BatchedMPC:
     reported as arrived).  With `enable_reverse` each waypoint carries a gear flag in its 4th row (+1 forward, -1
     reverse; mpc.py:139-144): every path is cut into single-gear curves (split_path, mpc.py:232-249), the solver's
     reference speed carries the gear's sign and a robot moves on to the next curve of its path when it reaches the end
-    of the current one (mpc.py:166-183).  cur_index is relative to the robot's curve, curve_index to its path."""
+    of the current one (mpc.py:166-183).  cur_index is relative to the robot's curve, curve_index to its path.
+
+    control(avoid_fleet=True) makes the robots that share a map obstacles of each other: every other robot of the
+    same map, its body at its current pose moving with the control it last applied, follows the map's shapes in the
+    list each robot chooses its N nearest obstacles from (convert_fleet_obstacles_batch)."""
 
     def __init__(self, car_tuple, ref_path, batch, receding=10, sample_time=0.1, iter_num=4,
                  enable_reverse=False, obstacle_order=True, max_edge_num=5, max_obs_num=5,
@@ -247,6 +328,9 @@ class BatchedMPC:
             self.cur_vel[:] = torch.as_tensor(init_vel, dtype=torch.float32, device=self.device)
         self.arrive = torch.zeros(batch, dtype=torch.int32, device=self.device)
         self._empty = None
+        self.body = robot_body(car_tuple)
+        self.body['xy'] = torch.as_tensor(self.body['xy'], device=self.device)
+        self._no_world = None
 
     def update_ref_path(self, ref_path, robot_path=None):
         """MPC.update_ref_path (mpc.py:220-227) for the whole fleet: replace the path set (one path, or W paths with
@@ -286,13 +370,26 @@ class BatchedMPC:
                            torch.zeros(B, dtype=torch.int32, device=dev))
         return self._empty
 
-    def control(self, state, ref_speed=5.0, shapes=None, time_varying=False, world=None, robot_world=None):
+    def control(self, state, ref_speed=5.0, shapes=None, time_varying=False, world=None, robot_world=None,
+                avoid_fleet=False):
         """state [B,3] (CUDA tensor or array), ref_speed scalar or [B], shapes: dict from
         pack_shapes / shapes_to_device (None: free space).  Instead of shapes, world: dict from
         pack_worlds / shapes_to_device, obstacle maps shared by the robots, with robot_world [B] the map of
-        each robot (may be omitted with a single map).  Returns (u0 [B,2], info) where info holds
-        the solver's batched outputs plus 'arrive', 'nom_s', 'ref_s', 'cur_index', 'curve_index'.  No host sync."""
+        each robot (may be omitted with a single map).  avoid_fleet: every robot also sees the other robots of its map
+        (without world: all robots, in an empty map) as moving obstacles; not with shapes.  Returns (u0 [B,2], info)
+        where info holds the solver's batched outputs plus 'arrive', 'nom_s', 'ref_s', 'cur_index', 'curve_index'.
+        No host sync."""
         dev, B, T = self.device, self.batch, self.T
+        if avoid_fleet:
+            if shapes is not None:
+                raise ValueError('avoid_fleet takes its obstacles from world= (or an empty map), not from shapes')
+            if self.body['kind'] == _cabi.OBS_POLYGON and self.body['nv'] > self.E:
+                raise ValueError(f'avoid_fleet: the robot body has {self.body["nv"]} vertices, more than '
+                                 f'max_edge_num={self.E} obstacle rows')
+            if world is None:
+                if self._no_world is None:
+                    self._no_world = shapes_to_device(pack_worlds([[]]), dev)
+                world = self._no_world
         if world is not None:
             if shapes is not None:
                 raise ValueError('pass either shapes or world, not both')
@@ -319,6 +416,10 @@ class BatchedMPC:
         if (shapes is None and world is None) or self.N == 0:
             A, b, kind, count = self._no_obstacles()
             time_varying = False
+        elif avoid_fleet:
+            fleet = fleet_shapes_batch(state, self.cur_vel, self.body, self.dynamics)
+            A, b, kind, count = convert_fleet_obstacles_batch(world, state, robot_world, fleet, self.N, T, self.E,
+                                                              self.dt, time_varying, self.obstacle_order)
         elif world is not None:
             A, b, kind, count = convert_world_obstacles_batch(world, state, robot_world, self.N, T, self.E, self.dt,
                                                               time_varying, self.obstacle_order)
