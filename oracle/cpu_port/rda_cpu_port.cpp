@@ -78,10 +78,20 @@ static int cell_dr_impl(const float* h, int kind, int E, const float* A, const f
   return 0;
 }
 
+// SeqCtx that also watches the su-QP's verification of the left-out hinges: its flag is the only integer that
+// su_solve reduces with max(), so the call tells whether the pruned attempt converged and was verified (a repeat
+// without that call was caused by the pruned attempt's iteration cap).  The solver's arithmetic is untouched.
+struct SuProbeCtx : SeqCtx {
+  mutable int verified = 0, violated = 0;
+  template <typename R> R max(R x) const { return x; }
+  int max(int x) const { ++verified; violated |= x; return x; }
+};
+
 template <typename Real>
 static int su_impl(const SuParams* P, const double* lins, const double* linu, const double* ref, double vref,
                    const double* dis, const float* hx, const float* hy, const float* hc, const float* gx,
-                   const float* gy, const double* pref, double* s, double* u, double* d, int* iters) {
+                   const float* gy, const double* pref, double* s, double* u, double* d, int* iters,
+                   int* report /* restarts, verifications, violation found; may be null */) {
   const int T = P->T, N = P->N;
   SuWork<Real> W;
   size_t bytes = su_work_bytes<Real>(T, N);
@@ -93,11 +103,12 @@ static int su_impl(const SuParams* P, const double* lins, const double* linu, co
   for (int i = 0; i < T; ++i) W.d[i] = (Real)dis[i];
   for (int i = 0; i < N * T; ++i) { W.hx[i] = hx[i]; W.hy[i] = hy[i]; W.hc[i] = hc[i]; }
   W.vref = (Real)vref;
-  SeqCtx ctx;
-  int st = su_solve<Real, SeqCtx>(*P, W, ctx, gx, gy, iters);
+  SuProbeCtx ctx;
+  int st = su_solve<Real, SuProbeCtx>(*P, W, ctx, gx, gy, iters);
   for (int i = 0; i < 3 * (T + 1); ++i) s[i] = W.s[i];
   for (int i = 0; i < 2 * T; ++i) u[i] = W.u[i];
   for (int i = 0; i < T; ++i) d[i] = W.d[i];
+  if (report) { report[0] = W.restarts; report[1] = ctx.verified; report[2] = ctx.violated; }
   return st;
 }
 
@@ -182,12 +193,23 @@ int shim_cell_dr_f(const float* h, int kind, int E, const float* A, const float*
 int shim_su_d(const SuParams* P, const double* lins, const double* linu, const double* ref, double vref,
               const double* dis, const float* hx, const float* hy, const float* hc, const float* gx,
               const float* gy, const double* pref, double* s, double* u, double* d, int* iters) {
-  return su_impl<double>(P, lins, linu, ref, vref, dis, hx, hy, hc, gx, gy, pref, s, u, d, iters);
+  return su_impl<double>(P, lins, linu, ref, vref, dis, hx, hy, hc, gx, gy, pref, s, u, d, iters, nullptr);
 }
 int shim_su_f(const SuParams* P, const double* lins, const double* linu, const double* ref, double vref,
               const double* dis, const float* hx, const float* hy, const float* hc, const float* gx,
               const float* gy, const double* pref, double* s, double* u, double* d, int* iters) {
-  return su_impl<float>(P, lins, linu, ref, vref, dis, hx, hy, hc, gx, gy, pref, s, u, d, iters);
+  return su_impl<float>(P, lins, linu, ref, vref, dis, hx, hy, hc, gx, gy, pref, s, u, d, iters, nullptr);
+}
+// as shim_su_*, plus report[3]: restarts, verifications of the left-out hinges, violation found (SuProbeCtx)
+int shim_su_report_d(const SuParams* P, const double* lins, const double* linu, const double* ref, double vref,
+                     const double* dis, const float* hx, const float* hy, const float* hc, const float* gx,
+                     const float* gy, const double* pref, double* s, double* u, double* d, int* iters, int* report) {
+  return su_impl<double>(P, lins, linu, ref, vref, dis, hx, hy, hc, gx, gy, pref, s, u, d, iters, report);
+}
+int shim_su_report_f(const SuParams* P, const double* lins, const double* linu, const double* ref, double vref,
+                     const double* dis, const float* hx, const float* hy, const float* hc, const float* gx,
+                     const float* gy, const double* pref, double* s, double* u, double* d, int* iters, int* report) {
+  return su_impl<float>(P, lins, linu, ref, vref, dis, hx, hy, hc, gx, gy, pref, s, u, d, iters, report);
 }
 }
 

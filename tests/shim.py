@@ -79,18 +79,29 @@ def cell_disc_robot(h, kind, A, b, p, phi, dbar, zeta, xi, ro2, theta=0.5, prec=
     return r
 
 
-def su(params, lins, linu, ref, vref, dis, hx, hy, hc, gx, gy, pref, prec='d'):
+def su(params, lins, linu, ref, vref, dis, hx, hy, hc, gx, gy, pref, prec='d', report=False):
+    """One su-QP solve: (s, u, d, status, interior point iterations); with report=True also a dict of the pruned
+    solve's repeat: restarts (1: repeated with all hinges), verified (the pruned attempt converged and its left-out
+    hinges were checked), violated (that check found one with l < 0), capped (the repeat was caused by the pruned
+    attempt's iteration cap, not by the check)."""
     T, N = params.T, params.N
     lins = _f64(np.asarray(lins).T); linu = _f64(np.asarray(linu).T); ref = _f64(np.asarray(ref).T)
     pref = _f64(np.asarray(pref).T); dis = _f64(np.ravel(dis))
     hx, hy, hc, gx, gy = (_f32(np.asarray(a).reshape(N, T)) for a in (hx, hy, hc, gx, gy))
     s = np.zeros((T + 1, 3)); u = np.zeros((T, 2)); d = np.zeros(T)
     it = C.c_int(0)
-    fn = getattr(lib(), 'shim_su_' + prec)
+    rep = np.zeros(3, np.int32)
+    fn = getattr(lib(), ('shim_su_report_' if report else 'shim_su_') + prec)
     fn.restype = C.c_int
+    extra = (_p(rep),) if report else ()
     st = fn(C.byref(params), _p(lins), _p(linu), _p(ref), C.c_double(vref), _p(dis), _p(hx), _p(hy), _p(hc),
-            _p(gx), _p(gy), _p(pref), _p(s), _p(u), _p(d), C.byref(it))
-    return s.T.copy(), u.T.copy(), d, st, it.value
+            _p(gx), _p(gy), _p(pref), _p(s), _p(u), _p(d), C.byref(it), *extra)
+    out = (s.T.copy(), u.T.copy(), d, st, it.value)
+    if not report:
+        return out
+    r = {'restarts': int(rep[0]), 'verified': int(rep[1]), 'violated': int(rep[2])}
+    r['capped'] = int(r['restarts'] == 1 and r['verified'] == 0)
+    return out + (r,)
 
 
 # ---- front end cores (frontend.cuh) ----
