@@ -57,6 +57,15 @@ typedef struct rda_tunables {   /* rda_solver.py:185-201, :426-434 */
   float z_theta;        /* tie-break of the slack z in [0, stuff] (DESIGN.md §3); 0.5 default */
 } rda_tunables;
 
+/* Columns of a per-instance parameter row (rda_set_instance_params): the limits and weights of rda_config and the
+ * tunables of rda_tunables that one instance of a batch may hold on its own.  z_theta, T, N, E, dt, the robot body
+ * and the dynamics stay per handle. */
+enum { RDA_IP_MAX_SPEED0 = 0, RDA_IP_MAX_SPEED1 = 1, /* rda_config.max_speed                   */
+       RDA_IP_ACCE_BOUND0 = 2, RDA_IP_ACCE_BOUND1 = 3, /* rda_config.acce_bound (max_acce * dt) */
+       RDA_IP_WS = 4, RDA_IP_WU = 5,                 /* rda_config.ws, wu                      */
+       RDA_IP_SLACK_GAIN = 6, RDA_IP_MAX_SD = 7, RDA_IP_MIN_SD = 8, RDA_IP_RO1 = 9, RDA_IP_RO2 = 10 };
+#define RDA_INST_PARAMS 11
+
 /* Inputs of one batched solve.  Layouts (row-major, last index fastest):
  *   nom_s  [B][3][T+1]   nominal states   (iterative_solve arg nom_s,  :573,:584)
  *   nom_u  [B][2][T]     nominal controls (arg nom_u)
@@ -90,6 +99,14 @@ int rda_destroy(rda_handle *h);
 /* assign_adjust_parameter (:426-434) / get_adjust_parameter (:1055-1056) */
 int rda_set_tunables(rda_handle *h, const rda_tunables *tun);
 int rda_get_tunables(const rda_handle *h, rda_tunables *tun);
+/* Per-instance limits, weights and tunables.  params: DEVICE pointer to float32 [B][RDA_INST_PARAMS]
+ * (column order RDA_IP_*), copied asynchronously on cuda_stream into storage the handle owns (allocated on the
+ * first call, freed by rda_destroy); from the next solve / phase call on, instance b uses row b instead of the
+ * handle's rda_config / rda_tunables values.  params = NULL: back to the handle's values for every instance.
+ * rda_set_tunables keeps updating the handle's values (rda_get_tunables returns them) while a table is installed,
+ * but the table wins for its columns; rda_reset and rda_cold_start leave the table alone.  The values are not
+ * checked: that is the caller's side (RDA_solver.set_instance_parameters). */
+int rda_set_instance_params(rda_handle *h, const float *params, void *cuda_stream);
 /* RDA_solver.reset (:1060-1068): clears lam'A and lam'b only. */
 int rda_reset(rda_handle *h, void *cuda_stream);
 /* Clear ALL warm-start state back to the constructor values (extension; used by benchmarks). */

@@ -16,6 +16,10 @@ ROBOT_POLYGON, ROBOT_DISC = 0, 1
 ST_SU_NOT_CONVERGED, ST_SU_NONFINITE, ST_CELL_FALLBACK, ST_EARLY_STOP = 1, 2, 4, 8
 (BUF_LAM, BUF_MU, BUF_Z, BUF_XI, BUF_ZETA, BUF_DIS, BUF_COEF, BUF_PREF, BUF_CUR_S, BUF_CUR_U,
  BUF_COUNTERS) = range(11)
+# columns of a per-instance parameter row (rda_set_instance_params)
+(IP_MAX_SPEED0, IP_MAX_SPEED1, IP_ACCE_BOUND0, IP_ACCE_BOUND1, IP_WS, IP_WU, IP_SLACK_GAIN, IP_MAX_SD, IP_MIN_SD, IP_RO1,
+ IP_RO2) = range(11)
+INST_PARAMS = 11
 
 
 class Config(C.Structure):
@@ -48,7 +52,8 @@ EXPORTS = ['rda_create', 'rda_destroy', 'rda_set_tunables', 'rda_get_tunables', 
            'rda_get_buffer', 'rda_copy_buffer', 'rda_last_launch_count', 'rda_version',
            'rda_pre_process', 'rda_convert_obstacles', 'rda_post_process', 'rda_motion_predict',
            'rda_pre_process_curves', 'rda_post_process_gear', 'rda_convert_world_obstacles',
-           'rda_pre_process_paths', 'rda_post_process_paths', 'rda_fleet_shapes', 'rda_convert_fleet_obstacles']
+           'rda_pre_process_paths', 'rda_post_process_paths', 'rda_fleet_shapes', 'rda_convert_fleet_obstacles',
+           'rda_set_instance_params']
 MAX_SHAPES = 64
 MAX_WORLD_SLOTS = 256
 
@@ -71,6 +76,7 @@ def load():
     lib.rda_destroy.argtypes = [vp]
     lib.rda_set_tunables.argtypes = [vp, C.POINTER(Tunables)]
     lib.rda_get_tunables.argtypes = [vp, C.POINTER(Tunables)]
+    lib.rda_set_instance_params.argtypes = [vp, vp, vp]
     lib.rda_reset.argtypes = [vp, vp]
     lib.rda_cold_start.argtypes = [vp, vp]
     lib.rda_solve.argtypes = [vp, C.POINTER(Inputs), C.POINTER(Outputs), C.c_int, C.c_float, vp]

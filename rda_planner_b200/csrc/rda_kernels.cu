@@ -78,6 +78,9 @@ struct rda_handle {
   int extra_min;             // sub-batches of at least this many instances run k_cells_extra before the cooperative pass (RDA_B200_EXTRA_MIN)
   int split_min;        // smallest batch that is split (RDA_B200_SPLIT_MIN, default 2048)
   int parts;             // number of sub-batches, 1..4 (RDA_B200_SPLIT_PARTS, default 2)
+  float* inst;           // [B][RDA_INST_PARAMS] per-instance limits, weights and tunables (rda_set_instance_params; allocated
+                         // on the first call), read by the kernels while inst_on is set
+  int inst_on;
 };
 
 #define RDA_CUDA(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) return (int)e_; } while (0)
@@ -122,6 +125,9 @@ struct DevPtrs {
   const int *obs_kind, *obs_count;
   int obs_tv;
   int B, T, N, E, R;
+  // per-instance limits, weights and tunables [B][RDA_INST_PARAMS] of this sub-batch (rda_set_instance_params), or
+  // nullptr: the handle's values (the launch arguments) for every instance
+  const float* inst;
 };
 
 __global__ void k_begin(DevPtrs d, const float* nom_s, const float* nom_u, const float* ref_s,
@@ -146,7 +152,9 @@ __global__ void k_begin(DevPtrs d, const float* nom_s, const float* nom_u, const
 // The su-QP of instance b: inputs from the persistent state (d), solve (su_solver.cuh), accepted result back.
 // W is laid out by the caller (hs / hnu and the workspace may live in shared or global memory).
 template <typename Real>
-__device__ __forceinline__ void su_instance(const DevPtrs& d, const SuParams& P, int b, SuWork<Real>& W, WarpCtx& ctx) {
+__device__ __forceinline__ void su_instance(const DevPtrs& d, const SuParams& Ph, int b, SuWork<Real>& W, WarpCtx& ctx) {
+  SuParams P = Ph;
+  if (d.inst) su_params_row(P, d.inst + (size_t)b * RDA_INST_PARAMS);     // the instance's own row
   const int T = P.T, N = P.N, NT = N * T;
   const int lane = ctx.lane();
   const float* cs = d.cur_s + (size_t)b * 3 * (T + 1);   // [3][T+1]
@@ -629,7 +637,7 @@ __device__ __forceinline__ void rows_preload(const DevPtrs& d, const CellIn& c, 
 
 // Second pass: the searched closed forms (vertex / edge contact, overlap cases) for the cells the first pass declined (records
 // in d.rec_b), one thread per record; the records of what is still unresolved go to d.rec_a.
-__global__ void __launch_bounds__(128) k_cells_mid(DevPtrs d, RobotGeom rb, float ro2, float theta) {
+__global__ void __launch_bounds__(128) k_cells_mid(DevPtrs d, RobotGeom rb, float ro2h, float theta) {
   const int count = d.wl_count[0];
   const int lane = threadIdx.x & 31;
   for (int base = blockIdx.x * blockDim.x; base < count; base += gridDim.x * blockDim.x) {
@@ -638,6 +646,7 @@ __global__ void __launch_bounds__(128) k_cells_mid(DevPtrs d, RobotGeom rb, floa
     bool need = false;
     if (live) {
       CellIn c = cell_from_rec(d, d.rec_b[wi]);
+      const float ro2 = inst_ro2(d.inst, c.b, ro2h);
       RowsLocal rows;
       rows_preload(d, c, rows);
       CellWork<float> w;
@@ -666,7 +675,7 @@ __global__ void __launch_bounds__(128) k_cells_mid(DevPtrs d, RobotGeom rb, floa
 // k_cells_dr_mid tries the searched closed forms of the listed cells, one cell per thread, and lists what is left in
 // d.rec_a; k_cells_dr_slow_coop runs the two-cone barrier programmes of those, one cell per warp.
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128) k_cells_dr(DevPtrs d, RobotGeom rb, float ro2, float theta) {
+__global__ void __launch_bounds__(128) k_cells_dr(DevPtrs d, RobotGeom rb, float ro2h, float theta) {
   const int NT = d.N * d.T;
   const long long total = (long long)d.B * NT;
   const int lane = threadIdx.x & 31;
@@ -678,6 +687,7 @@ __global__ void __launch_bounds__(128) k_cells_dr(DevPtrs d, RobotGeom rb, float
     bool need = false;
     if (live) {
       CellIn c = cell_load(d, idx);
+      const float ro2 = inst_ro2(d.inst, c.b, ro2h);
       CellWork<float> w;
       // first pass: the closed forms of the inactive hinge only (the searched ones run per listed cell in k_cells_dr_mid)
       cell_front_dr<float>(rb, c.kind, d.E, c.A, c.bb, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0, c.xi1, ro2, w, false);
@@ -701,13 +711,14 @@ __global__ void __launch_bounds__(128) k_cells_dr(DevPtrs d, RobotGeom rb, float
 // Disc body, second pass: the searched closed forms (edge and point contacts, overlap cases; point contacts in float64) for the
 // cells the first pass listed (records in d.rec_b), one thread per record; the records of what is left (0.01 % of the cells
 // on the bench workload) go to the cooperative barrier pass through d.rec_a.
-__global__ void __launch_bounds__(128) k_cells_dr_mid(DevPtrs d, RobotGeom rb, float ro2, float theta) {
+__global__ void __launch_bounds__(128) k_cells_dr_mid(DevPtrs d, RobotGeom rb, float ro2h, float theta) {
   const int count = d.wl_count[0];
   for (int base = blockIdx.x * blockDim.x; base < count; base += gridDim.x * blockDim.x) {
     const int wi = base + threadIdx.x;
     bool need = false;
     if (wi < count) {
       CellIn c = cell_from_rec(d, d.rec_b[wi]);
+      const float ro2 = inst_ro2(d.inst, c.b, ro2h);
       CellWork<float> w;
       cell_front_dr<float>(rb, c.kind, d.E, c.A, c.bb, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0, c.xi1, ro2, w, true);
       if (w.have) {
@@ -730,7 +741,7 @@ __global__ void __launch_bounds__(128) k_cells_dr_mid(DevPtrs d, RobotGeom rb, f
 constexpr int COOP_WARPS = 4;
 
 // one cell per WARP: the two-cone barrier iterations spread over the lanes, the problem in shared memory
-__global__ void __launch_bounds__(32 * COOP_WARPS) k_cells_dr_slow_coop(DevPtrs d, RobotGeom rb, float ro2, float theta) {
+__global__ void __launch_bounds__(32 * COOP_WARPS) k_cells_dr_slow_coop(DevPtrs d, RobotGeom rb, float ro2h, float theta) {
   __shared__ DiscSlowStore store[COOP_WARPS];
   const int count = d.wl_count[1];          // what k_cells_dr_mid left, in d.rec_a
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -742,6 +753,7 @@ __global__ void __launch_bounds__(32 * COOP_WARPS) k_cells_dr_slow_coop(DevPtrs 
     w.have = false;
     if (lane == 0) {
       c = cell_from_rec(d, d.rec_a[wi]);
+      const float ro2 = inst_ro2(d.inst, c.b, ro2h);
       // geometry only: the closed forms have been tried by k_cells_dr_mid
       cell_front_dr<float>(rb, c.kind, d.E, c.A, c.bb, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0, c.xi1, ro2, w, false);
     }
@@ -777,13 +789,14 @@ __global__ void __launch_bounds__(32 * COOP_WARPS) k_cells_dr_slow_coop(DevPtrs 
 // cell — they resolve ~90 % of that list; the records of what is left (~0.01 % of all cells) go to k_cells_slow_coop through
 // d.rec_b, which the searched pass has consumed by now.  (Doing these closed forms in lane 0 of the cooperative kernel was slow at
 // 16 384 unique instances: ten thousand warps each waiting for one serial lane.)
-__global__ void __launch_bounds__(128) k_cells_extra(DevPtrs d, RobotGeom rb, float ro2, float theta) {
+__global__ void __launch_bounds__(128) k_cells_extra(DevPtrs d, RobotGeom rb, float ro2h, float theta) {
   const int count = d.wl_count[1];
   for (int base = blockIdx.x * blockDim.x; base < count; base += gridDim.x * blockDim.x) {
     const int wi = base + threadIdx.x;
     bool need = false;
     if (wi < count) {
       CellIn c = cell_from_rec(d, d.rec_a[wi]);
+      const float ro2 = inst_ro2(d.inst, c.b, ro2h);
       RowsLocal rows;
       rows_preload(d, c, rows);
       CellWork<float> w;
@@ -808,7 +821,7 @@ __global__ void __launch_bounds__(128) k_cells_extra(DevPtrs d, RobotGeom rb, fl
 // vector components and Newton-matrix entries), the problem in shared memory.  Round 1 measured it slower than one thread per
 // cell — with 5 % of the cells in this pass; since the closed forms of round 2 leave 0.1 % (~13 000 cells at 16 384
 // instances, three waves of warps) the pass is a pure latency tail, which is what cooperation shortens (DESIGN.md §3.1).
-__global__ void __launch_bounds__(32 * COOP_WARPS) k_cells_slow_coop(DevPtrs d, RobotGeom rb, float ro2, float theta, int from_extra) {
+__global__ void __launch_bounds__(32 * COOP_WARPS) k_cells_slow_coop(DevPtrs d, RobotGeom rb, float ro2h, float theta, int from_extra) {
   __shared__ CellSlowStore store[COOP_WARPS];
   // from_extra: the records k_cells_extra left — d.rec_b (the first pass' list, consumed by now) with its own counter;
   // otherwise the searched pass' own leftovers in d.rec_a (small batches: one launch less, lane 0 runs the EXTRA closed forms)
@@ -823,6 +836,7 @@ __global__ void __launch_bounds__(32 * COOP_WARPS) k_cells_slow_coop(DevPtrs d, 
     w.have = false;
     if (lane == 0) {
       c = cell_from_rec(d, list[wi]);
+      const float ro2 = inst_ro2(d.inst, c.b, ro2h);
       cell_front<float, true>(rb, c.kind, d.E, c.A, c.bb, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0, c.xi1, ro2, w);
     }
     const int have = __shfl_sync(0xffffffffu, (int)w.have, 0);
@@ -941,16 +955,21 @@ __device__ __forceinline__ void bulk_commit_wait() {
 // Two resident CTAs per SM (small_max, and the staged state in shared memory): the register budget that leaves lets ptxas
 // keep the su-QP's working set in registers (without the bound it settles at 168 and spills in the float64 build).
 template <typename Real>
-__global__ void __launch_bounds__(128, 2) k_admm_small(DevPtrs d, SuParams P, RobotGeom rb, float ro2, float theta, float thr,
+__global__ void __launch_bounds__(128, 2) k_admm_small(DevPtrs d, SuParams Ph, RobotGeom rb, float theta, float thr,
                                                     int iter_num, SmallLayout L, const float* nom_s, const float* nom_u,
                                                     const float* ref_s, const float* ref_speed, rda_outputs out, int use_bulk) {
   extern __shared__ __align__(16) char smem[];
   const int b = blockIdx.x;
   if (b >= d.B) return;
   const int T = d.T, N = d.N, E = d.E, R = d.R, NT = N * T, tid = threadIdx.x, nth = blockDim.x;
+  // the su-QP parameters and the cells' ro2: the handle's, or the instance's own row (rda_set_instance_params), read once
+  SuParams P = Ph;
+  if (d.inst) su_params_row(P, d.inst + (size_t)b * RDA_INST_PARAMS);
+  const float ro2 = P.ro2;
   // ---- a one-instance view of the persistent state in shared memory ----
   DevPtrs ds = d;
   ds.B = 1;
+  ds.inst = nullptr;      // P holds the row
   ds.lam = (float*)(smem + L.lam); ds.mu = (float*)(smem + L.mu); ds.z = (float*)(smem + L.z); ds.xi = (float*)(smem + L.xi);
   ds.zeta = (float*)(smem + L.zeta); ds.dis = (float*)(smem + L.dis); ds.coef = (float*)(smem + L.coef);
   ds.pref = (float*)(smem + L.pref); ds.cur_s = (float*)(smem + L.cur_s); ds.cur_u = (float*)(smem + L.cur_u);
@@ -1171,6 +1190,7 @@ DevPtrs dev_ptrs(const rda_handle* h, int b0, int nb, int part) {
   d.obs_count = h->obs_count ? h->obs_count + o : nullptr;
   d.obs_tv = h->obs_tv;
   d.B = nb; d.T = h->T; d.N = h->N; d.E = h->E; d.R = h->R;
+  d.inst = h->inst_on ? h->inst + o * RDA_INST_PARAMS : nullptr;
   return d;
 }
 
@@ -1306,6 +1326,7 @@ int rda_destroy(rda_handle* h) {
   if (h->rec_a) cudaFree(h->rec_a);
   if (h->rec_b) cudaFree(h->rec_b);
   if (h->rot) cudaFree(h->rot);
+  if (h->inst) cudaFree(h->inst);
   if (h->ev_fork) cudaEventDestroy(h->ev_fork);
   for (int p = 0; p < 3; ++p) {
     if (h->ev_join[p]) cudaEventDestroy(h->ev_join[p]);
@@ -1324,6 +1345,16 @@ int rda_set_tunables(rda_handle* h, const rda_tunables* tun) {
 int rda_get_tunables(const rda_handle* h, rda_tunables* tun) {
   if (!h || !tun) return RDA_E_ARG;
   *tun = h->tun;
+  return 0;
+}
+
+int rda_set_instance_params(rda_handle* h, const float* params, void* stream) {
+  if (!h) return RDA_E_ARG;
+  if (!params) { h->inst_on = 0; return 0; }          // the storage stays for the next table
+  if (!h->inst) RDA_CUDA(cudaMalloc((void**)&h->inst, (size_t)h->B * RDA_INST_PARAMS * sizeof(float)));
+  RDA_CUDA(cudaMemcpyAsync(h->inst, params, (size_t)h->B * RDA_INST_PARAMS * sizeof(float), cudaMemcpyDeviceToDevice,
+                           (cudaStream_t)stream));
+  h->inst_on = 1;
   return 0;
 }
 
@@ -1519,11 +1550,11 @@ int rda_solve(rda_handle* h, const rda_inputs* in, const rda_outputs* out, int i
     SuParams P = su_params(h);
     const float theta = h->cfg.accelerated ? h->tun.z_theta : 1.0f;
     if (h->cfg.su_fp64)
-      k_admm_small<double><<<h->B, 128, h->small_L.total, s0>>>(d, P, h->rb, h->tun.ro2, theta, iter_threshold, iter_num, h->small_L,
+      k_admm_small<double><<<h->B, 128, h->small_L.total, s0>>>(d, P, h->rb, theta, iter_threshold, iter_num, h->small_L,
                                                               (const float*)in->nom_s, (const float*)in->nom_u, (const float*)in->ref_s,
                                                               (const float*)in->ref_speed, *out, h->small_bulk);
     else
-      k_admm_small<float><<<h->B, 128, h->small_L.total, s0>>>(d, P, h->rb, h->tun.ro2, theta, iter_threshold, iter_num, h->small_L,
+      k_admm_small<float><<<h->B, 128, h->small_L.total, s0>>>(d, P, h->rb, theta, iter_threshold, iter_num, h->small_L,
                                                              (const float*)in->nom_s, (const float*)in->nom_u, (const float*)in->ref_s,
                                                              (const float*)in->ref_speed, *out, h->small_bulk);
     RDA_CUDA(cudaGetLastError());

@@ -36,6 +36,20 @@ struct SuParams {
                   // the interior point iteration and verified afterwards (accelerated mode only); 0: keep all
 };
 
+// The su-QP parameters of one instance that has its own row of a per-instance table (rda_set_instance_params, columns
+// RDA_IP_*): the handle's P with the row's limits, weights and tunables.  The kernels (and the tests' CPU twin) select
+// with this.
+RDA_HD void su_params_row(SuParams& P, const float* row) {
+  P.umax[0] = row[RDA_IP_MAX_SPEED0]; P.umax[1] = row[RDA_IP_MAX_SPEED1];
+  P.ab[0] = row[RDA_IP_ACCE_BOUND0]; P.ab[1] = row[RDA_IP_ACCE_BOUND1];
+  P.ws = row[RDA_IP_WS]; P.wu = row[RDA_IP_WU];
+  P.slack_gain = row[RDA_IP_SLACK_GAIN]; P.dmax = row[RDA_IP_MAX_SD]; P.dmin = row[RDA_IP_MIN_SD];
+  P.ro1 = row[RDA_IP_RO1]; P.ro2 = row[RDA_IP_RO2];
+}
+
+// ADMM penalty ro2 of the cell passes: the instance's row when a table is installed, else the handle's value
+RDA_HD float inst_ro2(const float* inst, int b, float ro2) { return inst ? inst[(size_t)b * RDA_INST_PARAMS + RDA_IP_RO2] : ro2; }
+
 // Per-instance workspace.  All arrays indexed by stage t (0..T-1) unless noted; hinge planes (hx, hy, hc) indexed
 // [o*T + t], the compact hinge list (kx, ky, kc, hs, hnu) [k*T + t].  Real: arithmetic, iterate and slack / multiplier
 // type.

@@ -304,7 +304,10 @@ class BatchedMPC:
 
     control(avoid_fleet=True) makes the robots that share a map obstacles of each other: every other robot of the
     same map, its body at its current pose moving with the control it last applied, follows the map's shapes in the
-    list each robot chooses its N nearest obstacles from (convert_fleet_obstacles_batch)."""
+    list each robot chooses its N nearest obstacles from (convert_fleet_obstacles_batch).
+
+    update_parameter(robots=mask, max_speed=..., ro2=...) gives robots their own limits, weights and tunables, so that
+    robots of different classes (fast and slow, loaded and empty) step in one fleet and one solve."""
 
     def __init__(self, car_tuple, ref_path, batch, receding=10, sample_time=0.1, iter_num=4,
                  enable_reverse=False, obstacle_order=True, max_edge_num=5, max_obs_num=5,
@@ -360,6 +363,19 @@ class BatchedMPC:
         self.robot_path = torch.where(robots, robot_path, self.robot_path).contiguous()
         self.cur_index = self.cur_index.masked_fill(robots, 0)
         self.curve_index = self.curve_index.masked_fill(robots, 0)
+
+    def update_parameter(self, robots=None, **kwargs):
+        """MPC.update_parameter (mpc.py:229-230) for the whole fleet, or for the robots of the bool mask robots [B].
+        With scalar tunables and no mask this is exactly assign_adjust_parameter (slack_gain, max_sd, min_sd, ro1, ro2;
+        ws / wu ignored, as in the reference).  Otherwise the values go to the robots' own rows
+        (RDA_solver.set_instance_parameters): scalars or [B] / [B, 2] per robot, array-likes or CUDA tensors, and also
+        max_speed / max_acce (pairs) and ws / wu, so that one fleet can hold robots of different classes."""
+        uniform = robots is None and all(k not in ('max_speed', 'max_acce') and not isinstance(v, torch.Tensor)
+                                         and np.ndim(v) == 0 for k, v in kwargs.items())
+        if uniform:
+            self.rda.assign_adjust_parameter(**kwargs)
+        else:
+            self.rda.set_instance_parameters(robots, **kwargs)
 
     def _no_obstacles(self):
         if self._empty is None:

@@ -162,6 +162,86 @@ def pack_obstacles(obstacle_list, T, N, E, center=None, bound=None):
     return A, b, kind, count, tv
 
 
+# Per-instance parameters (RDA_solver.set_instance_parameters): key -> columns of the table (include/rda_b200.h, RDA_IP_*)
+INSTANCE_COLUMNS = {'max_speed': (_cabi.IP_MAX_SPEED0, _cabi.IP_MAX_SPEED1),
+                    'max_acce': (_cabi.IP_ACCE_BOUND0, _cabi.IP_ACCE_BOUND1),
+                    'ws': (_cabi.IP_WS,), 'wu': (_cabi.IP_WU,), 'slack_gain': (_cabi.IP_SLACK_GAIN,),
+                    'max_sd': (_cabi.IP_MAX_SD,), 'min_sd': (_cabi.IP_MIN_SD,), 'ro1': (_cabi.IP_RO1,),
+                    'ro2': (_cabi.IP_RO2,)}
+_POSITIVE = ('max_speed', 'max_acce', 'ro1', 'ro2')
+_NON_NEGATIVE = ('slack_gain', 'ws', 'wu')
+
+
+def _host_instance_value(key, value, B):
+    """A host-given per-instance value, checked: float64 array of shape () / (B,) (scalar keys) or (2,) / (B, 2)
+    (max_speed, max_acce)."""
+    a = np.asarray(value, dtype=float)
+    pair = len(INSTANCE_COLUMNS[key]) == 2
+    shapes = ((2,), (B, 2)) if pair else ((), (B,))
+    if a.shape not in shapes:
+        raise ValueError(f'{key}: expected shape {" or ".join(str(x) for x in shapes)}, got {a.shape}')
+    if not np.all(np.isfinite(a)):
+        raise ValueError(f'{key}: values must be finite')
+    if key in _POSITIVE and not np.all(a > 0):
+        raise ValueError(f'{key}: values must be > 0')
+    if key in _NON_NEGATIVE and not np.all(a >= 0):
+        raise ValueError(f'{key}: values must be >= 0')
+    return a
+
+
+def update_instance_table(table, dt, robots=None, validate=True, **values):
+    """A per-instance parameter table float32 [B, RDA_INST_PARAMS] (columns RDA_IP_*) with `values` written into the
+    rows of the bool mask `robots` [B] (None: every row); returns a new tensor on table's device, the input is left as
+    it is.  Keys of INSTANCE_COLUMNS; each value is a scalar (a pair for max_speed / max_acce) for every selected row,
+    or [B] ([B, 2]) per row, as an array-like or a tensor.  max_acce is stored as acce_bound = max_acce * dt, formed in
+    float64 and rounded to float32 as the constructor does.  Host-given values are checked (finite; max_speed,
+    max_acce, ro1, ro2 > 0; slack_gain, ws, wu >= 0; min_sd <= max_sd when both are given); tensors only for shape and
+    dtype, so that a call whose values and mask are all device tensors never waits for the device."""
+    B, dev = table.shape[0], table.device
+    unknown = sorted(set(values) - set(INSTANCE_COLUMNS))
+    if unknown:
+        raise TypeError(f'unknown per-instance parameter(s) {unknown}; known: {sorted(INSTANCE_COLUMNS)}')
+    if robots is not None:
+        robots = torch.as_tensor(robots, device=dev)
+        if robots.dtype != torch.bool or robots.shape != (B,):
+            raise ValueError(f'robots: expected a bool mask of shape ({B},), got {robots.dtype} {tuple(robots.shape)}')
+    host = {}
+    cols = {}       # column -> python float or float32 tensor [B]
+    for key, v in values.items():
+        pair = len(INSTANCE_COLUMNS[key]) == 2
+        if isinstance(v, torch.Tensor):
+            shapes = ((2,), (B, 2)) if pair else ((), (B,))
+            if tuple(v.shape) not in shapes or not v.is_floating_point():
+                raise ValueError(f'{key}: expected a floating tensor of shape {" or ".join(str(x) for x in shapes)}, '
+                                 f'got {v.dtype} {tuple(v.shape)}')
+            v = v.to(device=dev, dtype=torch.float64)
+            if key == 'max_acce':
+                v = v * float(dt)
+            v = v.to(torch.float32)
+            for j, c in enumerate(INSTANCE_COLUMNS[key]):
+                x = v[..., j] if pair else v
+                cols[c] = x.expand(B) if x.dim() == 0 else x
+            continue
+        a = _host_instance_value(key, v, B) if validate else np.asarray(v, dtype=float)
+        host[key] = a
+        if key == 'max_acce':
+            a = a * float(dt)
+        a = a.astype(np.float32)
+        for j, c in enumerate(INSTANCE_COLUMNS[key]):
+            x = a[..., j] if pair else a
+            cols[c] = float(x) if x.ndim == 0 else torch.as_tensor(x, device=dev)
+    if validate and 'min_sd' in host and 'max_sd' in host:
+        if not np.all(np.broadcast_to(host['min_sd'], (B,)) <= np.broadcast_to(host['max_sd'], (B,))):
+            raise ValueError('min_sd must not exceed max_sd')
+    out = table.clone()
+    for c, x in cols.items():
+        if robots is None:
+            out[:, c] = x
+        else:
+            out[:, c] = torch.where(robots, x, out[:, c])
+    return out
+
+
 class RDA_solver:
     def __init__(self, receding, car_tuple, max_edge_num=5, max_obs_num=5, iter_num=2, step_time=0.1,
                  iter_threshold=0.2, process_num=4, accelerated=True, time_print=True, batch=1,
@@ -249,6 +329,7 @@ class RDA_solver:
         self.use_graph = bool(graph)
         self._graphs = {}
         self._static = None
+        self._inst = None           # the installed per-instance table [B, RDA_INST_PARAMS] (set_instance_parameters)
 
     def __del__(self):
         try:
@@ -271,6 +352,58 @@ class RDA_solver:
             if k in kwargs:
                 self._tun_py[k] = kwargs[k]
         _cabi.check(self.lib.rda_set_tunables(self._h, C.byref(t)), 'rda_set_tunables')
+        if self._inst is not None:
+            # what the reference's update_parameter does on every robot's MPC: the named tunables of every instance
+            named = {k: float(getattr(t, k)) for k in self._tun_py if k in kwargs}
+            if named:
+                self._install(update_instance_table(self._inst, self.dt, validate=False, **named))
+
+    # ------------------------------------------------------------------ per-instance parameters
+    def _uniform_table(self):
+        """The handle's current limits, weights and tunables as a table [B, RDA_INST_PARAMS] on the device (column
+        fills, no host-to-device copy)."""
+        cfg, t = self._cfg, self._tun
+        row = [cfg.max_speed[0], cfg.max_speed[1], cfg.acce_bound[0], cfg.acce_bound[1], cfg.ws, cfg.wu,
+               t.slack_gain, t.max_sd, t.min_sd, t.ro1, t.ro2]
+        table = torch.empty((self.batch, _cabi.INST_PARAMS), dtype=torch.float32, device=self.device)
+        for c, v in enumerate(row):
+            table[:, c] = float(v)
+        return table
+
+    def _install(self, table):
+        with torch.cuda.device(self.device):
+            _cabi.check(self.lib.rda_set_instance_params(self._h, C.c_void_p(table.data_ptr()), self._stream()),
+                        'rda_set_instance_params')
+        if self._inst is None:
+            self._graphs.clear()        # captured launches carry "no table"; an update of an installed table is seen
+        self._inst = table              # the copy into the handle's storage reads it on the current stream
+
+    def set_instance_parameters(self, robots=None, **values):
+        """Give instances their own limits, weights and tunables: max_speed, max_acce (pairs), ws, wu, slack_gain,
+        max_sd, min_sd, ro1, ro2 — each a scalar (pair) for every selected instance or [B] ([B, 2]) per instance, as
+        an array-like or a CUDA tensor; robots: bool mask [B] that restricts the update (None: all).  The first call
+        starts from the handle's current values.  From the next solve on, instance b solves with its row as if it had
+        been constructed with those values (update_instance_table gives the checks).  Without host synchronisation when
+        every value and the mask are CUDA tensors."""
+        base = self._inst if self._inst is not None else self._uniform_table()
+        self._install(update_instance_table(base, self.dt, robots, **values))
+
+    def clear_instance_parameters(self):
+        """Back to the handle's values (constructor / assign_adjust_parameter) for every instance."""
+        with torch.cuda.device(self.device):
+            _cabi.check(self.lib.rda_set_instance_params(self._h, None, self._stream()), 'rda_set_instance_params')
+        if self._inst is not None:
+            self._graphs.clear()
+        self._inst = None
+
+    def instance_parameters(self):
+        """The values each instance solves with, dict of CUDA tensors: max_speed, acce_bound, max_acce (acce_bound / dt)
+        [B, 2] and ws, wu, slack_gain, max_sd, min_sd, ro1, ro2 [B]."""
+        table = self._inst if self._inst is not None else self._uniform_table()
+        out = {k: table[:, list(c)] if len(c) == 2 else table[:, c[0]] for k, c in INSTANCE_COLUMNS.items()}
+        out['acce_bound'] = out.pop('max_acce')
+        out['max_acce'] = (out['acce_bound'].double() / self.dt).float()
+        return {k: v.clone() for k, v in out.items()}
 
     def get_adjust_parameter(self):
         t = _cabi.Tunables()
