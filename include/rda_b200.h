@@ -58,13 +58,24 @@ typedef struct rda_tunables {   /* rda_solver.py:185-201, :426-434 */
 } rda_tunables;
 
 /* Columns of a per-instance parameter row (rda_set_instance_params): the limits and weights of rda_config and the
- * tunables of rda_tunables that one instance of a batch may hold on its own.  z_theta, T, N, E, dt, the robot body
- * and the dynamics stay per handle. */
+ * tunables of rda_tunables that one instance of a batch may hold on its own.  The body, wheelbase and dynamics come
+ * per instance from a robot class (rda_set_robot_classes); only z_theta, T, N, E, dt, the robot cone and R stay per
+ * handle. */
 enum { RDA_IP_MAX_SPEED0 = 0, RDA_IP_MAX_SPEED1 = 1, /* rda_config.max_speed                   */
        RDA_IP_ACCE_BOUND0 = 2, RDA_IP_ACCE_BOUND1 = 3, /* rda_config.acce_bound (max_acce * dt) */
        RDA_IP_WS = 4, RDA_IP_WU = 5,                 /* rda_config.ws, wu                      */
        RDA_IP_SLACK_GAIN = 6, RDA_IP_MAX_SD = 7, RDA_IP_MIN_SD = 8, RDA_IP_RO1 = 9, RDA_IP_RO2 = 10 };
 #define RDA_INST_PARAMS 11
+
+/* A robot class: the part of a car_tuple (G h cone_type wheelbase max_speed max_acce dynamics) that the per-instance
+ * parameter table does not hold.  G and h use the handle's robot_edges rows and robot_cone, as in rda_config. */
+#define RDA_MAX_ROBOT_CLASSES 16
+typedef struct rda_robot_class {
+  int dynamics;                    /* RDA_DYN_*                                   */
+  float wheelbase;                 /* L; > 0 for RDA_DYN_ACKER                    */
+  float G[RDA_MAX_ROBOT_EDGE * 2]; /* robot half-spaces, rows CCW                 */
+  float h[RDA_MAX_ROBOT_EDGE];
+} rda_robot_class;
 
 /* Inputs of one batched solve.  Layouts (row-major, last index fastest):
  *   nom_s  [B][3][T+1]   nominal states   (iterative_solve arg nom_s,  :573,:584)
@@ -107,6 +118,23 @@ int rda_get_tunables(const rda_handle *h, rda_tunables *tun);
  * but the table wins for its columns; rda_reset and rda_cold_start leave the table alone.  The values are not
  * checked: that is the caller's side (RDA_solver.set_instance_parameters). */
 int rda_set_instance_params(rda_handle *h, const float *params, void *cuda_stream);
+/* Robot classes of the handle: classes[0..K) (HOST array, read before the call returns) are checked and uploaded into
+ * device storage the handle owns (allocated on the first call for RDA_MAX_ROBOT_CLASSES, freed by rda_destroy).  Each
+ * class must have the handle's robot_cone and robot_edges rows; a disc class may have its own centre and radius.  A set-up
+ * call: ordered on cuda_stream, not graph-capturable.  K = 0 removes the classes.  Returns RDA_E_ARG for K outside
+ * [0, RDA_MAX_ROBOT_CLASSES], dynamics outside RDA_DYN_*, a non-finite wheelbase or an acker class with wheelbase <= 0;
+ * RDA_E_UNSUPPORTED for a body the handle's cone and row count cannot take.  Nothing is installed on an error. */
+int rda_set_robot_classes(rda_handle *h, int K, const rda_robot_class *classes, void *cuda_stream);
+/* The kernel variant (with or without classes) and K are fixed in the launches when a solve is recorded into a CUDA
+ * graph: a graph captured before the first rda_set_robot_class_index, after rda_set_robot_class_index(NULL), or before
+ * rda_set_robot_classes changed K must be captured again.  A new index copied into the same storage is seen by a
+ * replay. */
+/* The class of each instance: robot_class is a DEVICE pointer to int32 [B], copied asynchronously on cuda_stream into
+ * storage the handle owns (graph-capturable).  From the next solve / phase call on, instance b solves with the body,
+ * wheelbase and dynamics of class robot_class[b]; an index outside [0, K) means the handle's own rda_config body,
+ * wheelbase and dynamics (decided on the device).  robot_class = NULL: the handle's own for every instance.
+ * rda_reset and rda_cold_start leave the classes and the index alone. */
+int rda_set_robot_class_index(rda_handle *h, const int32_t *robot_class, void *cuda_stream);
 /* RDA_solver.reset (:1060-1068): clears lam'A and lam'b only. */
 int rda_reset(rda_handle *h, void *cuda_stream);
 /* Clear ALL warm-start state back to the constructor values (extension; used by benchmarks). */
@@ -222,6 +250,13 @@ int rda_convert_world_obstacles(int B, int W, int N, int T, int E, float dt, int
 int rda_fleet_shapes(int B, int T, int dynamics, int body_kind, int body_nv, const float *body_xy,
                      float body_radius, const float *state, const float *cur_vel, int32_t *shape_kind,
                      int32_t *shape_nv, float *shape_xy, float *shape_radius, float *shape_vel, void *cuda_stream);
+/* rda_fleet_shapes for a fleet of several robot classes: dynamics int32 [B], body_xy float32 [B][RDA_MAX_EDGE][2]
+ * (polygon: the body_nv vertices, disc: the centre in row 0) and body_radius float32 [B] per robot (device).  The kind
+ * and vertex count stay one per fleet, as the handle's cone and R do.  dynamics values are the caller's to check. */
+int rda_fleet_shapes_per_robot(int B, int T, const int32_t *dynamics, int body_kind, int body_nv, const float *body_xy,
+                               const float *body_radius, const float *state, const float *cur_vel, int32_t *shape_kind,
+                               int32_t *shape_nv, float *shape_xy, float *shape_radius, float *shape_vel,
+                               void *cuda_stream);
 int rda_convert_fleet_obstacles(int B, int W, int N, int T, int E, float dt, int time_varying, int order,
                                 const float *state, const int32_t *world_start, const int32_t *robot_world,
                                 const int32_t *shape_kind, const int32_t *shape_nv, const float *shape_xy,
@@ -280,6 +315,14 @@ int rda_pre_process_paths(int B, int T, int dynamics, float dt, float wheelbase,
                           const int32_t *robot_path, const int32_t *curve_index, const int32_t *start_index,
                           float threshold, int ind_range, float *nom_s, float *ref_s, int32_t *near_index,
                           float *solver_speed, void *cuda_stream);
+/* rda_pre_process_paths with each robot's own dynamics (int32 [B], RDA_DYN_*) and wheelbase (float32 [B]), device
+ * arrays (robot classes); the scalar entry point is this one with uniform arrays. */
+int rda_pre_process_paths_per_robot(int B, int T, const int32_t *dynamics, float dt, const float *wheelbase,
+                                    const float *state, const float *cur_vel, const float *ref_speed, const float *path,
+                                    int W, const int32_t *path_curve, const int32_t *curve_start,
+                                    const int32_t *curve_gear, const int32_t *robot_path, const int32_t *curve_index,
+                                    const int32_t *start_index, float threshold, int ind_range, float *nom_s,
+                                    float *ref_s, int32_t *near_index, float *solver_speed, void *cuda_stream);
 int rda_post_process_paths(int B, int T, int W, const int32_t *path_curve, const int32_t *curve_start,
                            const int32_t *robot_path, int goal_index_threshold, int32_t *near_index,
                            int32_t *curve_index, float *u_opt, float *cur_vel, int32_t *arrive,
@@ -289,6 +332,9 @@ int rda_post_process_paths(int B, int T, int W, const int32_t *path_curve, const
  * u_opt [B][2][T] (mpc.py:293-336; what the examples' simulator does between control calls). */
 int rda_motion_predict(int B, int T, int dynamics, float dt, float wheelbase, const float *u_opt,
                        float *state, void *cuda_stream);
+/* rda_motion_predict with each robot's own dynamics (int32 [B]) and wheelbase (float32 [B]), device arrays. */
+int rda_motion_predict_per_robot(int B, int T, const int32_t *dynamics, float dt, const float *wheelbase,
+                                 const float *u_opt, float *state, void *cuda_stream);
 
 #ifdef __cplusplus
 }

@@ -13,6 +13,7 @@ MAX_ROBOT_EDGE = 8
 DYNAMICS = {'acker': 0, 'diff': 1, 'omni': 2}
 OBS_POLYGON, OBS_CIRCLE = 0, 1
 ROBOT_POLYGON, ROBOT_DISC = 0, 1
+E_ARG, E_UNSUPPORTED, E_NOMEM = -1, -2, -3
 ST_SU_NOT_CONVERGED, ST_SU_NONFINITE, ST_CELL_FALLBACK, ST_EARLY_STOP = 1, 2, 4, 8
 (BUF_LAM, BUF_MU, BUF_Z, BUF_XI, BUF_ZETA, BUF_DIS, BUF_COEF, BUF_PREF, BUF_CUR_S, BUF_CUR_U,
  BUF_COUNTERS) = range(11)
@@ -20,6 +21,7 @@ ST_SU_NOT_CONVERGED, ST_SU_NONFINITE, ST_CELL_FALLBACK, ST_EARLY_STOP = 1, 2, 4,
 (IP_MAX_SPEED0, IP_MAX_SPEED1, IP_ACCE_BOUND0, IP_ACCE_BOUND1, IP_WS, IP_WU, IP_SLACK_GAIN, IP_MAX_SD, IP_MIN_SD, IP_RO1,
  IP_RO2) = range(11)
 INST_PARAMS = 11
+MAX_ROBOT_CLASSES = 16
 
 
 class Config(C.Structure):
@@ -34,6 +36,11 @@ class Config(C.Structure):
 class Tunables(C.Structure):
     _fields_ = [('slack_gain', C.c_float), ('max_sd', C.c_float), ('min_sd', C.c_float),
                 ('ro1', C.c_float), ('ro2', C.c_float), ('z_theta', C.c_float)]
+
+
+class RobotClass(C.Structure):
+    _fields_ = [('dynamics', C.c_int), ('wheelbase', C.c_float), ('G', C.c_float * (MAX_ROBOT_EDGE * 2)),
+                ('h', C.c_float * MAX_ROBOT_EDGE)]
 
 
 class Inputs(C.Structure):
@@ -53,7 +60,8 @@ EXPORTS = ['rda_create', 'rda_destroy', 'rda_set_tunables', 'rda_get_tunables', 
            'rda_pre_process', 'rda_convert_obstacles', 'rda_post_process', 'rda_motion_predict',
            'rda_pre_process_curves', 'rda_post_process_gear', 'rda_convert_world_obstacles',
            'rda_pre_process_paths', 'rda_post_process_paths', 'rda_fleet_shapes', 'rda_convert_fleet_obstacles',
-           'rda_set_instance_params']
+           'rda_set_instance_params', 'rda_set_robot_classes', 'rda_set_robot_class_index',
+           'rda_pre_process_paths_per_robot', 'rda_motion_predict_per_robot', 'rda_fleet_shapes_per_robot']
 MAX_SHAPES = 64
 MAX_WORLD_SLOTS = 256
 
@@ -77,6 +85,8 @@ def load():
     lib.rda_set_tunables.argtypes = [vp, C.POINTER(Tunables)]
     lib.rda_get_tunables.argtypes = [vp, C.POINTER(Tunables)]
     lib.rda_set_instance_params.argtypes = [vp, vp, vp]
+    lib.rda_set_robot_classes.argtypes = [vp, C.c_int, C.POINTER(RobotClass), vp]
+    lib.rda_set_robot_class_index.argtypes = [vp, vp, vp]
     lib.rda_reset.argtypes = [vp, vp]
     lib.rda_cold_start.argtypes = [vp, vp]
     lib.rda_solve.argtypes = [vp, C.POINTER(Inputs), C.POINTER(Outputs), C.c_int, C.c_float, vp]
@@ -99,6 +109,10 @@ def load():
                                           vp]
     lib.rda_post_process_paths.argtypes = [i, i, i, vp, vp, vp, i, vp, vp, vp, vp, vp, vp]
     lib.rda_motion_predict.argtypes = [i, i, i, f, f, vp, vp, vp]
+    lib.rda_pre_process_paths_per_robot.argtypes = [i, i, vp, f, vp, vp, vp, vp, vp, i, vp, vp, vp, vp, vp, vp, f, i, vp,
+                                                    vp, vp, vp, vp]
+    lib.rda_motion_predict_per_robot.argtypes = [i, i, vp, f, vp, vp, vp, vp]
+    lib.rda_fleet_shapes_per_robot.argtypes = [i, i, vp, i, i, vp, vp, vp, vp] + [vp] * 6
     lib.rda_fleet_shapes.argtypes = [i, i, i, i, i, vp, f] + [vp] * 8
     lib.rda_convert_fleet_obstacles.argtypes = [i, i, i, i, i, f, i, i] + [vp] * 20
     for name in EXPORTS:

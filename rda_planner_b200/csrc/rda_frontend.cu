@@ -17,8 +17,10 @@ namespace {
 
 // MPC.pre_process on the single-gear curve each robot follows (mpc.py:139-144, :251-291), and the solver's reference
 // speed gear * ref_speed (mpc.py:161).  A robot whose path index is outside [0, W) has no path: its nominal rollout as
-// usual, a reference that holds its current state, near_index 0 and gear +1.
-__global__ void k_pre_process_paths(int B, int T, int dynamics, float dt, float L, const float* state,
+// usual, a reference that holds its current state, near_index 0 and gear +1.  dyn_b / L_b [B]: each robot's own dynamics
+// and wheelbase (robot classes), or NULL: the scalars for every robot.
+__global__ void k_pre_process_paths(int B, int T, int dynamics, float dt, float L, const int* dyn_b, const float* L_b,
+                                    const float* state,
                                     const float* cur_vel, const float* ref_speed, const float* path, int P, int W,
                                     int n_curves, const int* path_curve, const int* curve_start, const int* curve_gear,
                                     const int* robot_path, const int* curve_index, const int* start_index,
@@ -27,6 +29,8 @@ __global__ void k_pre_process_paths(int B, int T, int dynamics, float dt, float 
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
   const int w = robot_path ? robot_path[b] : 0;
+  if (dyn_b) dynamics = dyn_b[b];
+  if (L_b) L = L_b[b];
   const float* st = state + 3 * (size_t)b;
   const float* vel = cur_vel + (size_t)b * 2 * T;
   float* nom = nom_s + (size_t)b * 3 * (T + 1);
@@ -233,13 +237,18 @@ k_convert_world_obstacles(int B, int W, int N, int T, int E, float dt, int time_
 }
 
 // Each robot of a fleet as a raw shape for its map-mates (fleet_shape), one thread per robot: its body at its pose,
-// moving with the first control of cur_vel, the one rda_motion_predict moved it with.
+// moving with the first control of cur_vel, the one rda_motion_predict moved it with.  dyn_b [B], body_xy_b [B][8][2] and
+// body_radius_b [B]: each robot's own dynamics and body (robot classes), or NULL: the scalars / the one body for every robot.
 __global__ void k_fleet_shapes(int B, int T, int dynamics, int body_kind, int body_nv, const float* body_xy,
-                               float body_radius, const float* state, const float* cur_vel, int* shape_kind,
+                               float body_radius, const int* dyn_b, const float* body_xy_b, const float* body_radius_b,
+                               const float* state, const float* cur_vel, int* shape_kind,
                                int* shape_nv, float* shape_xy, float* shape_radius, float* shape_vel) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
   const float* u = cur_vel + (size_t)b * 2 * T;
+  if (dyn_b) dynamics = dyn_b[b];
+  if (body_xy_b) body_xy = body_xy_b + (size_t)b * RDA_MAX_EDGE * 2;
+  if (body_radius_b) body_radius = body_radius_b[b];
   fleet_shape(dynamics, body_kind, body_nv, body_xy, body_radius, state + 3 * (size_t)b, (double)u[0], (double)u[T],
               shape_kind + b, shape_nv + b, shape_xy + (size_t)b * RDA_MAX_EDGE * 2, shape_radius + b,
               shape_vel + 2 * (size_t)b);
@@ -274,9 +283,13 @@ __global__ void k_post_process_paths(int B, int T, int P, int W, int n_curves, c
   if (arrive) arrive[b] = arr ? 1 : 0;
 }
 
-__global__ void k_motion_predict(int B, int T, int dynamics, float dt, float L, const float* u_opt, float* state) {
+// dyn_b / L_b [B]: each robot's own dynamics and wheelbase, or NULL: the scalars for every robot
+__global__ void k_motion_predict(int B, int T, int dynamics, float dt, float L, const int* dyn_b, const float* L_b,
+                                 const float* u_opt, float* state) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
+  if (dyn_b) dynamics = dyn_b[b];
+  if (L_b) L = L_b[b];
   const double s[3] = {state[3 * b], state[3 * b + 1], state[3 * b + 2]};
   double o[3];
   motion_predict(dynamics, (double)dt, (double)L, s, (double)u_opt[(size_t)b * 2 * T], (double)u_opt[(size_t)b * 2 * T + T], o);
@@ -317,7 +330,7 @@ int rda_pre_process(int B, int T, int dynamics, float dt, float wheelbase, const
   if (B < 1 || T < 1 || P < 1 || dynamics < 0 || dynamics > 2) return RDA_E_ARG;
   if (!state || !cur_vel || !ref_speed || !path || !nom_s || !ref_s || !near_index) return RDA_E_ARG;
   k_pre_process_paths<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(
-      B, T, dynamics, dt, wheelbase, state, cur_vel, ref_speed, path, P, 1, 1, nullptr, nullptr, nullptr, nullptr,
+      B, T, dynamics, dt, wheelbase, nullptr, nullptr, state, cur_vel, ref_speed, path, P, 1, 1, nullptr, nullptr, nullptr, nullptr,
       nullptr, start_index, threshold, ind_range, nom_s, ref_s, near_index, nullptr);
   RDA_CUDA(cudaGetLastError());
   return 0;
@@ -330,7 +343,7 @@ int rda_pre_process_curves(int B, int T, int dynamics, float dt, float wheelbase
   if (B < 1 || T < 1 || n_curves < 1 || dynamics < 0 || dynamics > 2) return RDA_E_ARG;
   if (!state || !cur_vel || !ref_speed || !path || !curve_start || !curve_index || !nom_s || !ref_s || !near_index) return RDA_E_ARG;
   k_pre_process_paths<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(
-      B, T, dynamics, dt, wheelbase, state, cur_vel, ref_speed, path, 0, 1, n_curves, nullptr, curve_start, nullptr,
+      B, T, dynamics, dt, wheelbase, nullptr, nullptr, state, cur_vel, ref_speed, path, 0, 1, n_curves, nullptr, curve_start, nullptr,
       nullptr, curve_index, start_index, threshold, ind_range, nom_s, ref_s, near_index, nullptr);
   RDA_CUDA(cudaGetLastError());
   return 0;
@@ -345,8 +358,24 @@ int rda_pre_process_paths(int B, int T, int dynamics, float dt, float wheelbase,
   if (!state || !cur_vel || !ref_speed || !path || !path_curve || !curve_start || !curve_gear) return RDA_E_ARG;
   if (!nom_s || !ref_s || !near_index) return RDA_E_ARG;
   k_pre_process_paths<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(
-      B, T, dynamics, dt, wheelbase, state, cur_vel, ref_speed, path, 0, W, 0, path_curve, curve_start, curve_gear,
-      robot_path, curve_index, start_index, threshold, ind_range, nom_s, ref_s, near_index, solver_speed);
+      B, T, dynamics, dt, wheelbase, nullptr, nullptr, state, cur_vel, ref_speed, path, 0, W, 0, path_curve, curve_start,
+      curve_gear, robot_path, curve_index, start_index, threshold, ind_range, nom_s, ref_s, near_index, solver_speed);
+  RDA_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int rda_pre_process_paths_per_robot(int B, int T, const int32_t* dynamics, float dt, const float* wheelbase,
+                                    const float* state, const float* cur_vel, const float* ref_speed, const float* path,
+                                    int W, const int32_t* path_curve, const int32_t* curve_start,
+                                    const int32_t* curve_gear, const int32_t* robot_path, const int32_t* curve_index,
+                                    const int32_t* start_index, float threshold, int ind_range, float* nom_s,
+                                    float* ref_s, int32_t* near_index, float* solver_speed, void* stream) {
+  if (B < 1 || T < 1 || W < 1 || !dynamics || !wheelbase) return RDA_E_ARG;
+  if (!state || !cur_vel || !ref_speed || !path || !path_curve || !curve_start || !curve_gear) return RDA_E_ARG;
+  if (!nom_s || !ref_s || !near_index) return RDA_E_ARG;
+  k_pre_process_paths<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(
+      B, T, 0, dt, 0.f, dynamics, wheelbase, state, cur_vel, ref_speed, path, 0, W, 0, path_curve, curve_start,
+      curve_gear, robot_path, curve_index, start_index, threshold, ind_range, nom_s, ref_s, near_index, solver_speed);
   RDA_CUDA(cudaGetLastError());
   return 0;
 }
@@ -411,8 +440,27 @@ int rda_fleet_shapes(int B, int T, int dynamics, int body_kind, int body_nv, con
   if (!body_xy || !state || !cur_vel || !shape_kind || !shape_nv || !shape_xy || !shape_radius || !shape_vel)
     return RDA_E_ARG;
   k_fleet_shapes<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(B, T, dynamics, body_kind, body_nv, body_xy,
-                                                                     body_radius, state, cur_vel, shape_kind, shape_nv,
-                                                                     shape_xy, shape_radius, shape_vel);
+                                                                     body_radius, nullptr, nullptr, nullptr, state, cur_vel,
+                                                                     shape_kind, shape_nv, shape_xy, shape_radius, shape_vel);
+  RDA_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int rda_fleet_shapes_per_robot(int B, int T, const int32_t* dynamics, int body_kind, int body_nv, const float* body_xy,
+                               const float* body_radius, const float* state, const float* cur_vel, int32_t* shape_kind,
+                               int32_t* shape_nv, float* shape_xy, float* shape_radius, float* shape_vel, void* stream) {
+  if (B < 1 || T < 1 || !dynamics) return RDA_E_ARG;
+  if (body_kind == RDA_OBS_POLYGON) {
+    if (body_nv < 3 || body_nv > RDA_MAX_EDGE) return RDA_E_UNSUPPORTED;
+  } else if (body_kind != RDA_OBS_CIRCLE) {
+    return RDA_E_ARG;
+  }
+  if (!body_xy || !body_radius || !state || !cur_vel || !shape_kind || !shape_nv || !shape_xy || !shape_radius ||
+      !shape_vel)
+    return RDA_E_ARG;
+  k_fleet_shapes<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(B, T, 0, body_kind, body_nv, nullptr, 0.f, dynamics,
+                                                                     body_xy, body_radius, state, cur_vel, shape_kind,
+                                                                     shape_nv, shape_xy, shape_radius, shape_vel);
   RDA_CUDA(cudaGetLastError());
   return 0;
 }
@@ -444,7 +492,16 @@ int rda_post_process(int B, int T, int P, int goal_index_threshold, const int32_
 int rda_motion_predict(int B, int T, int dynamics, float dt, float wheelbase, const float* u_opt, float* state,
                        void* stream) {
   if (B < 1 || T < 1 || dynamics < 0 || dynamics > 2 || !u_opt || !state) return RDA_E_ARG;
-  k_motion_predict<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(B, T, dynamics, dt, wheelbase, u_opt, state);
+  k_motion_predict<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(B, T, dynamics, dt, wheelbase, nullptr, nullptr,
+                                                                       u_opt, state);
+  RDA_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int rda_motion_predict_per_robot(int B, int T, const int32_t* dynamics, float dt, const float* wheelbase,
+                                 const float* u_opt, float* state, void* stream) {
+  if (B < 1 || T < 1 || !dynamics || !wheelbase || !u_opt || !state) return RDA_E_ARG;
+  k_motion_predict<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(B, T, 0, dt, 0.f, dynamics, wheelbase, u_opt, state);
   RDA_CUDA(cudaGetLastError());
   return 0;
 }

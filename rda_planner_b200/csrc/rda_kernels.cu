@@ -81,6 +81,15 @@ struct rda_handle {
   float* inst;           // [B][RDA_INST_PARAMS] per-instance limits, weights and tunables (rda_set_instance_params; allocated
                          // on the first call), read by the kernels while inst_on is set
   int inst_on;
+  // robot classes (rda_set_robot_classes; allocated on the first call): tables [RDA_MAX_ROBOT_CLASSES + 1] whose slot ncls
+  // holds the handle's own body, wheelbase and dynamics, and the class index [B] (rda_set_robot_class_index), read by
+  // the kernels while cls_on is set and ncls > 0
+  RobotGeom* cls_rb;
+  RobotAux* cls_ra;
+  ClassKin* cls_kin;
+  int ncls;
+  int* cls_idx;
+  int cls_on;
 };
 
 #define RDA_CUDA(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) return (int)e_; } while (0)
@@ -128,7 +137,30 @@ struct DevPtrs {
   // per-instance limits, weights and tunables [B][RDA_INST_PARAMS] of this sub-batch (rda_set_instance_params), or
   // nullptr: the handle's values (the launch arguments) for every instance
   const float* inst;
+  // the class index [B] of this sub-batch and the class tables [ncls + 1] (class_slot), or cls = nullptr: the
+  // handle's body, wheelbase and dynamics (the launch arguments) for every instance.  The cell passes are compiled
+  // for either case (template argument CLS, chosen at launch from cls).
+  const int* cls;
+  int ncls;
+  const RobotGeom* cls_rb;
+  const RobotAux* cls_ra;
+  const ClassKin* cls_kin;
 };
+
+// The body of the instance in class-table slot `slot` (slot_of): its class's with a class table (CLS), else the
+// handle's (rb, the launch argument).  Without a table the cells read the body from the kernel parameters as before.
+template <bool CLS> __device__ __forceinline__ int slot_of(const DevPtrs& d, int b) {
+  if constexpr (CLS) return class_slot(d.cls, d.ncls, b);
+  else return 0;
+}
+template <bool CLS> __device__ __forceinline__ const RobotGeom& body_at(const DevPtrs& d, const RobotGeom& rb, int slot) {
+  if constexpr (CLS) return d.cls_rb[slot];
+  else return rb;
+}
+template <bool CLS> __device__ __forceinline__ const RobotAux& aux_at(const DevPtrs& d, const RobotAux& ra, int slot) {
+  if constexpr (CLS) return d.cls_ra[slot];
+  else return ra;
+}
 
 __global__ void k_begin(DevPtrs d, const float* nom_s, const float* nom_u, const float* ref_s,
                         const float* ref_speed) {
@@ -155,6 +187,7 @@ template <typename Real>
 __device__ __forceinline__ void su_instance(const DevPtrs& d, const SuParams& Ph, int b, SuWork<Real>& W, WarpCtx& ctx) {
   SuParams P = Ph;
   if (d.inst) su_params_row(P, d.inst + (size_t)b * RDA_INST_PARAMS);     // the instance's own row
+  if (d.cls) su_params_class(P, d.cls_kin[class_slot(d.cls, d.ncls, b)]);  // its class's dynamics and wheelbase
   const int T = P.T, N = P.N, NT = N * T;
   const int lane = ctx.lane();
   const float* cs = d.cur_s + (size_t)b * 3 * (T + 1);   // [3][T+1]
@@ -375,8 +408,8 @@ __device__ __forceinline__ void cell_store(const DevPtrs& d, const CellIn& c, co
 // First pass: compile-time specialised lean solver (cell_lean.cuh), geometry in registers.
 // LISTED: the cells come from the records in d.rec_a (what the coherent pass k_cells_coh declined) instead of the whole
 // batch.  What this pass declines goes to d.rec_b as records.
-template <int EC, int RC, bool LISTED>
-__global__ void __launch_bounds__(128, (EC <= 4 ? 6 : 3)) k_cells_fast(DevPtrs d, RobotGeom rb, float theta) {
+template <int EC, int RC, bool LISTED, bool CLS>
+__global__ void __launch_bounds__(128, (EC <= 4 ? 6 : 3)) k_cells_fast(DevPtrs d, RobotGeom rbh, float theta) {
   const int T = d.T, N = d.N, E = d.E, R = d.R;
   const int NT = N * T;
   const long long total = LISTED ? (long long)d.wl_count[2] : (long long)d.B * NT;
@@ -393,6 +426,7 @@ __global__ void __launch_bounds__(128, (EC <= 4 ? 6 : 3)) k_cells_fast(DevPtrs d
     if (!LISTED && live && (d.done[b] || d.obs_count[b] == 0)) live = false;
     if (live) {
       CellIn c = LISTED ? cell_from_rec(d, rec) : cell_load(d, idx);
+      const RobotGeom& rb = body_at<CLS>(d, rbh, slot_of<CLS>(d, c.b));
       // issue every global load of this cell before the arithmetic (memory-level parallelism): the
       // obstacle rows (128-bit loads when E == 4) and the previous duals needed for the residual
       float Ar[2 * EC], br[EC], lamo[EC], muo[RC];
@@ -528,12 +562,18 @@ __global__ void k_heading(DevPtrs d, float* rot) {
 // `tiles` = ceil(cells of one instance / 128) CTAs per instance, instance-major (blockIdx.x = b * tiles + tile,
 // so any batch size fits; gridDim.y would cap it at 65 535) — no 64-bit index arithmetic, one instance per CTA
 // (uniform early exit, one residual atomic per warp), 32-bit offsets inside the instance.
-__global__ void __launch_bounds__(128, 6) k_cells_coh(DevPtrs d, RobotGeom rb, RobotAux ra, const float* __restrict__ rot,
+template <bool CLS>
+__global__ void __launch_bounds__(128, 6) k_cells_coh(DevPtrs d, RobotGeom rbh, RobotAux rah, const float* __restrict__ rot,
                                                       float theta, float invT, int tiles) {
   constexpr int EC = 4, RC = 4;
   const int T = d.T, N = d.N, E = d.E, R = d.R, NT = N * T;
   const int b = blockIdx.x / tiles;
   if (d.done[b] || d.obs_count[b] == 0) return;             // uniform for the CTA
+  // the body of the CTA's instance; the feat hint of a robot whose class changed is checked like any other
+  // (cell_lean2 accepts a pair only through the separating-slab certificate)
+  const int slot = slot_of<CLS>(d, b);
+  const RobotGeom& rb = body_at<CLS>(d, rbh, slot);
+  const RobotAux& ra = aux_at<CLS>(d, rah, slot);
   const int rem = (blockIdx.x - b * tiles) * blockDim.x + threadIdx.x;
   const int lane = threadIdx.x & 31;
   const bool live = rem < NT;
@@ -637,7 +677,8 @@ __device__ __forceinline__ void rows_preload(const DevPtrs& d, const CellIn& c, 
 
 // Second pass: the searched closed forms (vertex / edge contact, overlap cases) for the cells the first pass declined (records
 // in d.rec_b), one thread per record; the records of what is still unresolved go to d.rec_a.
-__global__ void __launch_bounds__(128) k_cells_mid(DevPtrs d, RobotGeom rb, float ro2h, float theta) {
+template <bool CLS>
+__global__ void __launch_bounds__(128) k_cells_mid(DevPtrs d, RobotGeom rbh, float ro2h, float theta) {
   const int count = d.wl_count[0];
   const int lane = threadIdx.x & 31;
   for (int base = blockIdx.x * blockDim.x; base < count; base += gridDim.x * blockDim.x) {
@@ -647,6 +688,7 @@ __global__ void __launch_bounds__(128) k_cells_mid(DevPtrs d, RobotGeom rb, floa
     if (live) {
       CellIn c = cell_from_rec(d, d.rec_b[wi]);
       const float ro2 = inst_ro2(d.inst, c.b, ro2h);
+      const RobotGeom& rb = body_at<CLS>(d, rbh, slot_of<CLS>(d, c.b));
       RowsLocal rows;
       rows_preload(d, c, rows);
       CellWork<float> w;
@@ -675,7 +717,8 @@ __global__ void __launch_bounds__(128) k_cells_mid(DevPtrs d, RobotGeom rb, floa
 // k_cells_dr_mid tries the searched closed forms of the listed cells, one cell per thread, and lists what is left in
 // d.rec_a; k_cells_dr_slow_coop runs the two-cone barrier programmes of those, one cell per warp.
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128) k_cells_dr(DevPtrs d, RobotGeom rb, float ro2h, float theta) {
+template <bool CLS>
+__global__ void __launch_bounds__(128) k_cells_dr(DevPtrs d, RobotGeom rbh, float ro2h, float theta) {
   const int NT = d.N * d.T;
   const long long total = (long long)d.B * NT;
   const int lane = threadIdx.x & 31;
@@ -688,6 +731,7 @@ __global__ void __launch_bounds__(128) k_cells_dr(DevPtrs d, RobotGeom rb, float
     if (live) {
       CellIn c = cell_load(d, idx);
       const float ro2 = inst_ro2(d.inst, c.b, ro2h);
+      const RobotGeom& rb = body_at<CLS>(d, rbh, slot_of<CLS>(d, c.b));
       CellWork<float> w;
       // first pass: the closed forms of the inactive hinge only (the searched ones run per listed cell in k_cells_dr_mid)
       cell_front_dr<float>(rb, c.kind, d.E, c.A, c.bb, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0, c.xi1, ro2, w, false);
@@ -711,7 +755,8 @@ __global__ void __launch_bounds__(128) k_cells_dr(DevPtrs d, RobotGeom rb, float
 // Disc body, second pass: the searched closed forms (edge and point contacts, overlap cases; point contacts in float64) for the
 // cells the first pass listed (records in d.rec_b), one thread per record; the records of what is left (0.01 % of the cells
 // on the bench workload) go to the cooperative barrier pass through d.rec_a.
-__global__ void __launch_bounds__(128) k_cells_dr_mid(DevPtrs d, RobotGeom rb, float ro2h, float theta) {
+template <bool CLS>
+__global__ void __launch_bounds__(128) k_cells_dr_mid(DevPtrs d, RobotGeom rbh, float ro2h, float theta) {
   const int count = d.wl_count[0];
   for (int base = blockIdx.x * blockDim.x; base < count; base += gridDim.x * blockDim.x) {
     const int wi = base + threadIdx.x;
@@ -719,6 +764,7 @@ __global__ void __launch_bounds__(128) k_cells_dr_mid(DevPtrs d, RobotGeom rb, f
     if (wi < count) {
       CellIn c = cell_from_rec(d, d.rec_b[wi]);
       const float ro2 = inst_ro2(d.inst, c.b, ro2h);
+      const RobotGeom& rb = body_at<CLS>(d, rbh, slot_of<CLS>(d, c.b));
       CellWork<float> w;
       cell_front_dr<float>(rb, c.kind, d.E, c.A, c.bb, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0, c.xi1, ro2, w, true);
       if (w.have) {
@@ -741,7 +787,8 @@ __global__ void __launch_bounds__(128) k_cells_dr_mid(DevPtrs d, RobotGeom rb, f
 constexpr int COOP_WARPS = 4;
 
 // one cell per WARP: the two-cone barrier iterations spread over the lanes, the problem in shared memory
-__global__ void __launch_bounds__(32 * COOP_WARPS) k_cells_dr_slow_coop(DevPtrs d, RobotGeom rb, float ro2h, float theta) {
+template <bool CLS>
+__global__ void __launch_bounds__(32 * COOP_WARPS) k_cells_dr_slow_coop(DevPtrs d, RobotGeom rbh, float ro2h, float theta) {
   __shared__ DiscSlowStore store[COOP_WARPS];
   const int count = d.wl_count[1];          // what k_cells_dr_mid left, in d.rec_a
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -751,8 +798,11 @@ __global__ void __launch_bounds__(32 * COOP_WARPS) k_cells_dr_slow_coop(DevPtrs 
     CellIn c;
     CellWork<float> w;
     w.have = false;
+    int slot = 0;
+    if (lane == 0) c = cell_from_rec(d, d.rec_a[wi]);
+    if (CLS) slot = __shfl_sync(0xffffffffu, slot_of<CLS>(d, lane == 0 ? c.b : 0), 0);   // every lane takes part in the barrier solve
+    const RobotGeom& rb = body_at<CLS>(d, rbh, slot);
     if (lane == 0) {
-      c = cell_from_rec(d, d.rec_a[wi]);
       const float ro2 = inst_ro2(d.inst, c.b, ro2h);
       // geometry only: the closed forms have been tried by k_cells_dr_mid
       cell_front_dr<float>(rb, c.kind, d.E, c.A, c.bb, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0, c.xi1, ro2, w, false);
@@ -789,7 +839,8 @@ __global__ void __launch_bounds__(32 * COOP_WARPS) k_cells_dr_slow_coop(DevPtrs 
 // cell — they resolve ~90 % of that list; the records of what is left (~0.01 % of all cells) go to k_cells_slow_coop through
 // d.rec_b, which the searched pass has consumed by now.  (Doing these closed forms in lane 0 of the cooperative kernel was slow at
 // 16 384 unique instances: ten thousand warps each waiting for one serial lane.)
-__global__ void __launch_bounds__(128) k_cells_extra(DevPtrs d, RobotGeom rb, float ro2h, float theta) {
+template <bool CLS>
+__global__ void __launch_bounds__(128) k_cells_extra(DevPtrs d, RobotGeom rbh, float ro2h, float theta) {
   const int count = d.wl_count[1];
   for (int base = blockIdx.x * blockDim.x; base < count; base += gridDim.x * blockDim.x) {
     const int wi = base + threadIdx.x;
@@ -797,6 +848,7 @@ __global__ void __launch_bounds__(128) k_cells_extra(DevPtrs d, RobotGeom rb, fl
     if (wi < count) {
       CellIn c = cell_from_rec(d, d.rec_a[wi]);
       const float ro2 = inst_ro2(d.inst, c.b, ro2h);
+      const RobotGeom& rb = body_at<CLS>(d, rbh, slot_of<CLS>(d, c.b));
       RowsLocal rows;
       rows_preload(d, c, rows);
       CellWork<float> w;
@@ -821,7 +873,8 @@ __global__ void __launch_bounds__(128) k_cells_extra(DevPtrs d, RobotGeom rb, fl
 // vector components and Newton-matrix entries), the problem in shared memory.  Round 1 measured it slower than one thread per
 // cell — with 5 % of the cells in this pass; since the closed forms of round 2 leave 0.1 % (~13 000 cells at 16 384
 // instances, three waves of warps) the pass is a pure latency tail, which is what cooperation shortens (DESIGN.md §3.1).
-__global__ void __launch_bounds__(32 * COOP_WARPS) k_cells_slow_coop(DevPtrs d, RobotGeom rb, float ro2h, float theta, int from_extra) {
+template <bool CLS>
+__global__ void __launch_bounds__(32 * COOP_WARPS) k_cells_slow_coop(DevPtrs d, RobotGeom rbh, float ro2h, float theta, int from_extra) {
   __shared__ CellSlowStore store[COOP_WARPS];
   // from_extra: the records k_cells_extra left — d.rec_b (the first pass' list, consumed by now) with its own counter;
   // otherwise the searched pass' own leftovers in d.rec_a (small batches: one launch less, lane 0 runs the EXTRA closed forms)
@@ -834,8 +887,11 @@ __global__ void __launch_bounds__(32 * COOP_WARPS) k_cells_slow_coop(DevPtrs d, 
     CellIn c;
     CellWork<float> w;
     w.have = false;
+    int slot = 0;
+    if (lane == 0) c = cell_from_rec(d, list[wi]);
+    if (CLS) slot = __shfl_sync(0xffffffffu, slot_of<CLS>(d, lane == 0 ? c.b : 0), 0);   // every lane takes part in the interior point solve
+    const RobotGeom& rb = body_at<CLS>(d, rbh, slot);
     if (lane == 0) {
-      c = cell_from_rec(d, list[wi]);
       const float ro2 = inst_ro2(d.inst, c.b, ro2h);
       cell_front<float, true>(rb, c.kind, d.E, c.A, c.bb, c.px, c.py, c.cp, c.sp, c.dbar, c.zeta, c.xi0, c.xi1, ro2, w);
     }
@@ -864,8 +920,9 @@ __global__ void __launch_bounds__(32 * COOP_WARPS) k_cells_slow_coop(DevPtrs d, 
 }
 
 // per instance: residuals (:688, :735-739), early stop (:594-596), empty-list quirk (:564-568)
-__device__ __forceinline__ void finalize_instance(const DevPtrs& d, const RobotGeom& rb, float thr, int b) {
+__device__ __forceinline__ void finalize_instance(const DevPtrs& d, const RobotGeom& rbh, float thr, int b) {
   const int T = d.T, N = d.N, NT = N * T, R = d.R;
+  const float* rh = d.cls ? d.cls_rb[class_slot(d.cls, d.ncls, b)].h : rbh.h;
   float pri = 0.f, dual = 0.f;
   if (N > 0 && d.obs_count[b] != 0) {
     pri = sqrtf(d.resi_acc[2 * b]);
@@ -877,7 +934,7 @@ __device__ __forceinline__ void finalize_instance(const DevPtrs& d, const RobotG
     for (int t = 0; t < T; ++t) {
       const float* mu = d.mu + ((size_t)b * N + o) * R * T + t;
       float muh = 0.f;
-      for (int j = 0; j < R; ++j) muh += mu[(size_t)j * T] * rb.h[j];
+      for (int j = 0; j < R; ++j) muh += mu[(size_t)j * T] * rh[j];
       size_t cell = (size_t)b * NT + (size_t)o * T + t;
       cf[t] = 0.f; cf[NT + t] = 0.f;
       cf[2 * NT + t] = -muh - d.z[cell] + d.zeta[cell];
@@ -954,8 +1011,8 @@ __device__ __forceinline__ void bulk_commit_wait() {
 
 // Two resident CTAs per SM (small_max, and the staged state in shared memory): the register budget that leaves lets ptxas
 // keep the su-QP's working set in registers (without the bound it settles at 168 and spills in the float64 build).
-template <typename Real>
-__global__ void __launch_bounds__(128, 2) k_admm_small(DevPtrs d, SuParams Ph, RobotGeom rb, float theta, float thr,
+template <typename Real, bool CLS>
+__global__ void __launch_bounds__(128, 2) k_admm_small(DevPtrs d, SuParams Ph, RobotGeom rbh, float theta, float thr,
                                                     int iter_num, SmallLayout L, const float* nom_s, const float* nom_u,
                                                     const float* ref_s, const float* ref_speed, rda_outputs out, int use_bulk) {
   extern __shared__ __align__(16) char smem[];
@@ -966,10 +1023,15 @@ __global__ void __launch_bounds__(128, 2) k_admm_small(DevPtrs d, SuParams Ph, R
   SuParams P = Ph;
   if (d.inst) su_params_row(P, d.inst + (size_t)b * RDA_INST_PARAMS);
   const float ro2 = P.ro2;
+  // the body, dynamics and wheelbase: the handle's, or the instance's class (rda_set_robot_classes), read once
+  const int slot = slot_of<CLS>(d, b);
+  const RobotGeom& rb = body_at<CLS>(d, rbh, slot);
+  if (CLS) su_params_class(P, d.cls_kin[slot]);
   // ---- a one-instance view of the persistent state in shared memory ----
   DevPtrs ds = d;
   ds.B = 1;
   ds.inst = nullptr;      // P holds the row
+  ds.cls = nullptr;       // ... and the class's kinematics; rb is its body
   ds.lam = (float*)(smem + L.lam); ds.mu = (float*)(smem + L.mu); ds.z = (float*)(smem + L.z); ds.xi = (float*)(smem + L.xi);
   ds.zeta = (float*)(smem + L.zeta); ds.dis = (float*)(smem + L.dis); ds.coef = (float*)(smem + L.coef);
   ds.pref = (float*)(smem + L.pref); ds.cur_s = (float*)(smem + L.cur_s); ds.cur_u = (float*)(smem + L.cur_u);
@@ -1148,7 +1210,7 @@ __global__ void k_finish(DevPtrs d, rda_outputs o) {
 }
 
 // RDA_solver.reset (:1060-1068): lam'A = 0, lam'b = 0; mu, z, zeta, xi are NOT cleared.
-__global__ void k_reset(DevPtrs d, RobotGeom rb) {
+__global__ void k_reset(DevPtrs d, RobotGeom rbh) {
   const int T = d.T, N = d.N, NT = N * T, R = d.R;
   const long long total = (long long)d.B * NT;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
@@ -1156,8 +1218,9 @@ __global__ void k_reset(DevPtrs d, RobotGeom rb) {
     int rem = (int)(idx - (long long)b * NT);
     int o = rem / T, t = rem - o * T;
     const float* mu = d.mu + ((size_t)b * N + o) * R * T + t;
+    const float* rh = d.cls ? d.cls_rb[class_slot(d.cls, d.ncls, b)].h : rbh.h;
     float muh = 0.f;
-    for (int j = 0; j < R; ++j) muh += mu[(size_t)j * T] * rb.h[j];
+    for (int j = 0; j < R; ++j) muh += mu[(size_t)j * T] * rh[j];
     float* cf = d.coef + (size_t)b * 5 * NT + rem;
     cf[0] = 0.f; cf[NT] = 0.f;
     cf[2 * NT] = -muh - d.z[idx] + d.zeta[idx];
@@ -1191,6 +1254,8 @@ DevPtrs dev_ptrs(const rda_handle* h, int b0, int nb, int part) {
   d.obs_tv = h->obs_tv;
   d.B = nb; d.T = h->T; d.N = h->N; d.E = h->E; d.R = h->R;
   d.inst = h->inst_on ? h->inst + o * RDA_INST_PARAMS : nullptr;
+  d.cls = h->cls_on && h->ncls > 0 ? h->cls_idx + o : nullptr;
+  d.ncls = h->ncls; d.cls_rb = h->cls_rb; d.cls_ra = h->cls_ra; d.cls_kin = h->cls_kin;
   return d;
 }
 
@@ -1210,6 +1275,9 @@ SuParams su_params(const rda_handle* h) {
   P.prune = h->su_prune;
   return P;
 }
+
+// the variant of a kernel for the sub-batch d: with a class table or without (DevPtrs::cls)
+template <typename K> K by_cls(const DevPtrs& d, K with_classes, K without) { return d.cls ? with_classes : without; }
 
 int grid_for(long long n, int block, int sms) {
   long long g = (n + block - 1) / block;
@@ -1297,8 +1365,14 @@ int rda_create(const rda_config* cfg, const rda_tunables* tun, rda_handle** out)
     if (const char* v = getenv("RDA_B200_SMALL")) { int x = atoi(v); if (x >= -1 && x <= 1) h->small_mode = x; }
     if (const char* v = getenv("RDA_B200_SMALL_MAX")) { int x = atoi(v); if (x >= 1) h->small_max = x; }
     if (h->small_ok) {
-      if (cfg->su_fp64) e = cudaFuncSetAttribute(k_admm_small<double>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->small_L.total);
-      else e = cudaFuncSetAttribute(k_admm_small<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, h->small_L.total);
+      for (int c = 0; c < 2 && e == cudaSuccess; ++c) {
+        if (cfg->su_fp64)
+          e = cudaFuncSetAttribute(c ? k_admm_small<double, true> : k_admm_small<double, false>,
+                                   cudaFuncAttributeMaxDynamicSharedMemorySize, h->small_L.total);
+        else
+          e = cudaFuncSetAttribute(c ? k_admm_small<float, true> : k_admm_small<float, false>,
+                                   cudaFuncAttributeMaxDynamicSharedMemorySize, h->small_L.total);
+      }
       if (e != cudaSuccess) { rda_destroy(h); return (int)e; }
     }
   }
@@ -1327,6 +1401,10 @@ int rda_destroy(rda_handle* h) {
   if (h->rec_b) cudaFree(h->rec_b);
   if (h->rot) cudaFree(h->rot);
   if (h->inst) cudaFree(h->inst);
+  if (h->cls_rb) cudaFree(h->cls_rb);
+  if (h->cls_ra) cudaFree(h->cls_ra);
+  if (h->cls_kin) cudaFree(h->cls_kin);
+  if (h->cls_idx) cudaFree(h->cls_idx);
   if (h->ev_fork) cudaEventDestroy(h->ev_fork);
   for (int p = 0; p < 3; ++p) {
     if (h->ev_join[p]) cudaEventDestroy(h->ev_join[p]);
@@ -1355,6 +1433,51 @@ int rda_set_instance_params(rda_handle* h, const float* params, void* stream) {
   RDA_CUDA(cudaMemcpyAsync(h->inst, params, (size_t)h->B * RDA_INST_PARAMS * sizeof(float), cudaMemcpyDeviceToDevice,
                            (cudaStream_t)stream));
   h->inst_on = 1;
+  return 0;
+}
+
+int rda_set_robot_classes(rda_handle* h, int K, const rda_robot_class* classes, void* stream) {
+  if (!h || K < 0 || K > RDA_MAX_ROBOT_CLASSES || (K > 0 && !classes)) return RDA_E_ARG;
+  // slots 0..K-1: the classes, slot K: the handle's own body (an index outside [0, K))
+  RobotGeom rb[RDA_MAX_ROBOT_CLASSES + 1];
+  RobotAux ra[RDA_MAX_ROBOT_CLASSES + 1];
+  ClassKin kin[RDA_MAX_ROBOT_CLASSES + 1];
+  for (int k = 0; k < K; ++k) {
+    const rda_robot_class& c = classes[k];
+    if (c.dynamics < RDA_DYN_ACKER || c.dynamics > RDA_DYN_OMNI || !isfinite(c.wheelbase)) return RDA_E_ARG;
+    if (c.dynamics == RDA_DYN_ACKER && !(c.wheelbase > 0.f)) return RDA_E_ARG;
+  }
+  for (int k = 0; k < K; ++k) {
+    const int rc = robot_geom_from_halfspaces(classes[k].G, classes[k].h, h->R, &rb[k], h->cfg.robot_cone);
+    if (rc) return rc;
+    kin[k].dynamics = classes[k].dynamics; kin[k].L = classes[k].wheelbase;
+  }
+  rb[K] = h->rb;
+  kin[K].dynamics = h->cfg.dynamics; kin[K].L = h->cfg.wheelbase;
+  for (int k = 0; k <= K; ++k) {
+    if (rb[k].disc) memset(&ra[k], 0, sizeof(RobotAux));      // the coherent pass, the only reader, takes polygons only
+    else robot_aux_from_geom(rb[k], &ra[k]);
+  }
+  const size_t n = RDA_MAX_ROBOT_CLASSES + 1;
+  if (!h->cls_rb) RDA_CUDA(cudaMalloc((void**)&h->cls_rb, n * sizeof(RobotGeom)));
+  if (!h->cls_ra) RDA_CUDA(cudaMalloc((void**)&h->cls_ra, n * sizeof(RobotAux)));
+  if (!h->cls_kin) RDA_CUDA(cudaMalloc((void**)&h->cls_kin, n * sizeof(ClassKin)));
+  cudaStream_t s = (cudaStream_t)stream;
+  // pageable host source: each copy has read it when the call returns
+  RDA_CUDA(cudaMemcpyAsync(h->cls_rb, rb, (K + 1) * sizeof(RobotGeom), cudaMemcpyHostToDevice, s));
+  RDA_CUDA(cudaMemcpyAsync(h->cls_ra, ra, (K + 1) * sizeof(RobotAux), cudaMemcpyHostToDevice, s));
+  RDA_CUDA(cudaMemcpyAsync(h->cls_kin, kin, (K + 1) * sizeof(ClassKin), cudaMemcpyHostToDevice, s));
+  h->ncls = K;
+  return 0;
+}
+
+int rda_set_robot_class_index(rda_handle* h, const int32_t* robot_class, void* stream) {
+  if (!h) return RDA_E_ARG;
+  if (!robot_class) { h->cls_on = 0; return 0; }     // the storage stays for the next index
+  if (!h->cls_idx) RDA_CUDA(cudaMalloc((void**)&h->cls_idx, (size_t)h->B * sizeof(int)));
+  RDA_CUDA(cudaMemcpyAsync(h->cls_idx, robot_class, (size_t)h->B * sizeof(int), cudaMemcpyDeviceToDevice,
+                           (cudaStream_t)stream));
+  h->cls_on = 1;
   return 0;
 }
 
@@ -1430,11 +1553,11 @@ static int step_lammuz_part(rda_handle* h, int b0, int nb, int part, cudaStream_
   if (h->N > 0) {
     const float theta = h->cfg.accelerated ? h->tun.z_theta : 1.0f;
     if (h->rb.disc) {
-      k_cells_dr<<<grid_for((long long)nb * h->N * h->T, 128, h->sms), 128, 0, s>>>(d, h->rb, h->tun.ro2, theta);
+      by_cls(d, k_cells_dr<true>, k_cells_dr<false>)<<<grid_for((long long)nb * h->N * h->T, 128, h->sms), 128, 0, s>>>(d, h->rb, h->tun.ro2, theta);
       RDA_CUDA(cudaGetLastError());
-      k_cells_dr_mid<<<h->sms * 8, 128, 0, s>>>(d, h->rb, h->tun.ro2, theta);
+      by_cls(d, k_cells_dr_mid<true>, k_cells_dr_mid<false>)<<<h->sms * 8, 128, 0, s>>>(d, h->rb, h->tun.ro2, theta);
       RDA_CUDA(cudaGetLastError());
-      k_cells_dr_slow_coop<<<h->sms * 16, 32 * COOP_WARPS, 0, s>>>(d, h->rb, h->tun.ro2, theta);
+      by_cls(d, k_cells_dr_slow_coop<true>, k_cells_dr_slow_coop<false>)<<<h->sms * 16, 32 * COOP_WARPS, 0, s>>>(d, h->rb, h->tun.ro2, theta);
       RDA_CUDA(cudaGetLastError());
       h->launches += 3;
       k_finalize<<<(nb + 127) / 128, 128, 0, s>>>(d, h->rb, h->iter_threshold);
@@ -1446,27 +1569,27 @@ static int step_lammuz_part(rda_handle* h, int b0, int nb, int part, cudaStream_
       k_heading<<<(nb * h->T + 255) / 256, 256, 0, s>>>(d, h->rot + (size_t)b0 * 2 * h->T);
       RDA_CUDA(cudaGetLastError());
       const int tiles = (h->N * h->T + 127) / 128;
-      k_cells_coh<<<(unsigned)tiles * (unsigned)nb, 128, 0, s>>>(d, h->rb, h->ra, h->rot + (size_t)b0 * 2 * h->T, theta,
+      by_cls(d, k_cells_coh<true>, k_cells_coh<false>)<<<(unsigned)tiles * (unsigned)nb, 128, 0, s>>>(d, h->rb, h->ra, h->rot + (size_t)b0 * 2 * h->T, theta,
                                                                 1.0f / (float)h->T, tiles);
       h->launches += 1;
       RDA_CUDA(cudaGetLastError());
-      k_cells_fast<4, 4, true><<<grid_for((long long)nb * h->N * h->T, 128, h->sms), 128, 0, s>>>(d, h->rb, theta);
+      by_cls(d, k_cells_fast<4, 4, true, true>, k_cells_fast<4, 4, true, false>)<<<grid_for((long long)nb * h->N * h->T, 128, h->sms), 128, 0, s>>>(d, h->rb, theta);
       h->launches += 1;
     } else if (h->E <= 4 && h->R <= 4)
-      k_cells_fast<4, 4, false><<<grid_for((long long)nb * h->N * h->T, 128, h->sms), 128, 0, s>>>(d, h->rb, theta);
+      by_cls(d, k_cells_fast<4, 4, false, true>, k_cells_fast<4, 4, false, false>)<<<grid_for((long long)nb * h->N * h->T, 128, h->sms), 128, 0, s>>>(d, h->rb, theta);
     else
-      k_cells_fast<8, 8, false><<<grid_for((long long)nb * h->N * h->T, 128, h->sms), 128, 0, s>>>(d, h->rb, theta);
+      by_cls(d, k_cells_fast<8, 8, false, true>, k_cells_fast<8, 8, false, false>)<<<grid_for((long long)nb * h->N * h->T, 128, h->sms), 128, 0, s>>>(d, h->rb, theta);
     RDA_CUDA(cudaGetLastError());
-    k_cells_mid<<<h->sms * 16, 128, 0, s>>>(d, h->rb, h->tun.ro2, theta);     // a few waves of the 6 resident CTAs per SM
+    by_cls(d, k_cells_mid<true>, k_cells_mid<false>)<<<h->sms * 16, 128, 0, s>>>(d, h->rb, h->tun.ro2, theta);     // a few waves of the 6 resident CTAs per SM
     RDA_CUDA(cudaGetLastError());
     // the split costs a launch and pays from a few thousand instances on
     const int split = nb >= h->extra_min;
     if (split) {
-      k_cells_extra<<<h->sms * 4, 128, 0, s>>>(d, h->rb, h->tun.ro2, theta);
+      by_cls(d, k_cells_extra<true>, k_cells_extra<false>)<<<h->sms * 4, 128, 0, s>>>(d, h->rb, h->tun.ro2, theta);
       RDA_CUDA(cudaGetLastError());
       h->launches += 1;
     }
-    k_cells_slow_coop<<<h->sms * 16, 32 * COOP_WARPS, 0, s>>>(d, h->rb, h->tun.ro2, theta, split);
+    by_cls(d, k_cells_slow_coop<true>, k_cells_slow_coop<false>)<<<h->sms * 16, 32 * COOP_WARPS, 0, s>>>(d, h->rb, h->tun.ro2, theta, split);
     RDA_CUDA(cudaGetLastError());
     h->launches += 3;
   }
@@ -1550,11 +1673,11 @@ int rda_solve(rda_handle* h, const rda_inputs* in, const rda_outputs* out, int i
     SuParams P = su_params(h);
     const float theta = h->cfg.accelerated ? h->tun.z_theta : 1.0f;
     if (h->cfg.su_fp64)
-      k_admm_small<double><<<h->B, 128, h->small_L.total, s0>>>(d, P, h->rb, theta, iter_threshold, iter_num, h->small_L,
+      by_cls(d, k_admm_small<double, true>, k_admm_small<double, false>)<<<h->B, 128, h->small_L.total, s0>>>(d, P, h->rb, theta, iter_threshold, iter_num, h->small_L,
                                                               (const float*)in->nom_s, (const float*)in->nom_u, (const float*)in->ref_s,
                                                               (const float*)in->ref_speed, *out, h->small_bulk);
     else
-      k_admm_small<float><<<h->B, 128, h->small_L.total, s0>>>(d, P, h->rb, theta, iter_threshold, iter_num, h->small_L,
+      by_cls(d, k_admm_small<float, true>, k_admm_small<float, false>)<<<h->B, 128, h->small_L.total, s0>>>(d, P, h->rb, theta, iter_threshold, iter_num, h->small_L,
                                                              (const float*)in->nom_s, (const float*)in->nom_u, (const float*)in->ref_s,
                                                              (const float*)in->ref_speed, *out, h->small_bulk);
     RDA_CUDA(cudaGetLastError());

@@ -50,6 +50,16 @@ RDA_HD void su_params_row(SuParams& P, const float* row) {
 // ADMM penalty ro2 of the cell passes: the instance's row when a table is installed, else the handle's value
 RDA_HD float inst_ro2(const float* inst, int b, float ro2) { return inst ? inst[(size_t)b * RDA_INST_PARAMS + RDA_IP_RO2] : ro2; }
 
+// Kinematics of a robot class (rda_set_robot_classes) as the handle's class table keeps them.
+struct ClassKin { int dynamics; float L; };
+
+// Slot of instance b in the handle's class tables [K + 1]: its class index when that is in [0, K), else K, the slot that
+// holds the handle's own body, wheelbase and dynamics.  The kernels (and the tests' CPU twin) select with this.
+RDA_HD int class_slot(const int* cls, int K, int b) { const int k = cls[b]; return (k >= 0 && k < K) ? k : K; }
+
+// The su-QP parameters of an instance of a robot class: the handle's P with the class's dynamics and wheelbase.
+RDA_HD void su_params_class(SuParams& P, const ClassKin& k) { P.dynamics = k.dynamics; P.L = k.L; }
+
 // Per-instance workspace.  All arrays indexed by stage t (0..T-1) unless noted; hinge planes (hx, hy, hc) indexed
 // [o*T + t], the compact hinge list (kx, ky, kc, hs, hnu) [k*T + t].  Real: arithmetic, iterate and slack / multiplier
 // type.

@@ -230,11 +230,12 @@ def robot_body(car_tuple):
     return {'kind': _cabi.OBS_POLYGON, 'nv': len(V), 'xy': xy, 'radius': 0.0}
 
 
-def fleet_shapes_batch(state, cur_vel, body, dynamics):
+def fleet_shapes_batch(state, cur_vel, body, dynamics, per_robot=None):
     """CUDA tensors state [B,3], cur_vel [B,2,T] (the controls each robot last applied in cur_vel[:, :, 0]); body from
     robot_body with xy a CUDA tensor.  Returns every robot as one raw shape for its map-mates, dict of CUDA tensors in
     the layout of pack_worlds without 'start': its body at its pose, moving with the world-frame velocity of its
-    control."""
+    control.  per_robot: None, or a dict of CUDA tensors 'dynamics' int32 [B], 'xy' float32 [B,8,2] and 'radius' float32
+    [B], each robot's own dynamics and body (robot classes; body gives the kind and vertex count of every robot)."""
     lib = _cabi.load()
     dev = state.device
     B, T = state.shape[0], cur_vel.shape[2]
@@ -242,6 +243,14 @@ def fleet_shapes_batch(state, cur_vel, body, dynamics):
            'xy': torch.empty((B, _cabi.MAX_EDGE, 2), dtype=torch.float32, device=dev),
            'radius': torch.empty(B, dtype=torch.float32, device=dev),
            'vel': torch.empty((B, 2), dtype=torch.float32, device=dev)}
+    if per_robot is not None:
+        with torch.cuda.device(dev):
+            _cabi.check(lib.rda_fleet_shapes_per_robot(B, T, _ptr(per_robot['dynamics']), body['kind'], body['nv'],
+                                                       _ptr(per_robot['xy']), _ptr(per_robot['radius']), _ptr(state),
+                                                       _ptr(cur_vel), _ptr(out['kind']), _ptr(out['nv']), _ptr(out['xy']),
+                                                       _ptr(out['radius']), _ptr(out['vel']), _stream(dev)),
+                        'rda_fleet_shapes_per_robot')
+        return out
     with torch.cuda.device(dev):
         _cabi.check(lib.rda_fleet_shapes(B, T, _cabi.DYNAMICS[dynamics], body['kind'], body['nv'], _ptr(body['xy']),
                                          body['radius'], _ptr(state), _ptr(cur_vel), _ptr(out['kind']), _ptr(out['nv']),
@@ -307,13 +316,25 @@ class BatchedMPC:
     list each robot chooses its N nearest obstacles from (convert_fleet_obstacles_batch).
 
     update_parameter(robots=mask, max_speed=..., ro2=...) gives robots their own limits, weights and tunables, so that
-    robots of different classes (fast and slow, loaded and empty) step in one fleet and one solve."""
+    robots of different classes (fast and slow, loaded and empty) step in one fleet and one solve.
+
+    With `robot_class` [B], car_tuple is a list of up to 16 car_tuples (robot classes of one cone_type and one number of
+    canonical body rows) and robot b is of class robot_class[b]: its body, wheelbase, dynamics and limits (and its body
+    and motion as others see it with avoid_fleet).  The handle is built with class 0, so an index outside the list means
+    class 0.  set_robot_class moves robots between classes on the device."""
 
     def __init__(self, car_tuple, ref_path, batch, receding=10, sample_time=0.1, iter_num=4,
                  enable_reverse=False, obstacle_order=True, max_edge_num=5, max_obs_num=5,
-                 accelerated=True, goal_index_threshold=1, device=None, iter_threshold=0.2, robot_path=None, **kwargs):
+                 accelerated=True, goal_index_threshold=1, device=None, iter_threshold=0.2, robot_path=None,
+                 robot_class=None, **kwargs):
         self.lib = _cabi.load()
         self.enable_reverse = bool(enable_reverse)
+        self.classes = None
+        if robot_class is not None:
+            self.classes = list(car_tuple)
+            if not self.classes:
+                raise ValueError('robot_class needs at least one car_tuple')
+            car_tuple = self.classes[0]
         self.rda = RDA_solver(receding, car_tuple, max_edge_num, max_obs_num, iter_num=iter_num,
                               step_time=sample_time, iter_threshold=iter_threshold, accelerated=accelerated,
                               time_print=False, batch=batch, device=device, **kwargs)
@@ -334,6 +355,35 @@ class BatchedMPC:
         self.body = robot_body(car_tuple)
         self.body['xy'] = torch.as_tensor(self.body['xy'], device=self.device)
         self._no_world = None
+        self.per_robot = None
+        if self.classes is not None:
+            self.rda.set_robot_classes(self.classes, robot_class)
+            bodies = [robot_body(c) for c in self.classes + [car_tuple]]
+            self._class_nv = max(int(bd['nv']) for bd in bodies)
+            dev = self.device
+            # per class slot [K + 1] (slot K: class 0, the handle's own), uploaded once
+            self._class_tables = {
+                'dynamics': torch.tensor([_cabi.DYNAMICS[c.dynamics] for c in self.classes + [car_tuple]],
+                                         dtype=torch.int32, device=dev),
+                'wheelbase': torch.tensor([float(c.wheelbase) for c in self.classes + [car_tuple]], dtype=torch.float32,
+                                          device=dev),
+                'xy': torch.as_tensor(np.stack([bd['xy'] for bd in bodies]), device=dev),
+                'radius': torch.tensor([bd['radius'] for bd in bodies], dtype=torch.float32, device=dev)}
+            self._gather_classes()
+
+    def _gather_classes(self):
+        """Each robot's dynamics, wheelbase and body from its class, gathered on the device."""
+        slot = self.rda.class_slot()
+        self.per_robot = {k: v[slot].contiguous() for k, v in self._class_tables.items()}
+
+    def set_robot_class(self, index, robots):
+        """Move the robots of the bool mask robots [B] to class index ([B] or one index; outside the classes: class 0):
+        their body, wheelbase, dynamics, max_speed and max_acce change from the next control call, their warm start is
+        kept.  On the device, without a host synchronisation when index and robots are CUDA tensors."""
+        if self.classes is None:
+            raise RuntimeError('set_robot_class needs a fleet built with robot_class')
+        self.rda.set_robot_class_index(index, torch.as_tensor(robots, dtype=torch.bool, device=self.device))
+        self._gather_classes()
 
     def update_ref_path(self, ref_path, robot_path=None):
         """MPC.update_ref_path (mpc.py:220-227) for the whole fleet: replace the path set (one path, or W paths with
@@ -399,8 +449,9 @@ class BatchedMPC:
         if avoid_fleet:
             if shapes is not None:
                 raise ValueError('avoid_fleet takes its obstacles from world= (or an empty map), not from shapes')
-            if self.body['kind'] == _cabi.OBS_POLYGON and self.body['nv'] > self.E:
-                raise ValueError(f'avoid_fleet: the robot body has {self.body["nv"]} vertices, more than '
+            nv = self.body['nv'] if self.classes is None else self._class_nv
+            if self.body['kind'] == _cabi.OBS_POLYGON and nv > self.E:
+                raise ValueError(f'avoid_fleet: a robot body has {nv} vertices, more than '
                                  f'max_edge_num={self.E} obstacle rows')
             if world is None:
                 if self._no_world is None:
@@ -422,18 +473,24 @@ class BatchedMPC:
         ref_s = torch.empty((B, 3, T + 1), dtype=torch.float32, device=dev)
         near = torch.empty(B, dtype=torch.int32, device=dev)
         solver_speed = torch.empty(B, dtype=torch.float32, device=dev)          # gear_flag * ref_speed (mpc.py:161)
+        paths = (_ptr(self.path), self.n_paths, _ptr(self.path_curve), _ptr(self.curve_start), _ptr(self.curve_gear),
+                 _ptr(self.robot_path), _ptr(self.curve_index), _ptr(self.cur_index), 0.1, 10, _ptr(nom_s), _ptr(ref_s),
+                 _ptr(near), _ptr(solver_speed), _stream(dev))
         with torch.cuda.device(dev):
-            _cabi.check(self.lib.rda_pre_process_paths(
-                B, T, _cabi.DYNAMICS[self.dynamics], self.dt, self.L, _ptr(state), _ptr(self.cur_vel), _ptr(ref_speed),
-                _ptr(self.path), self.n_paths, _ptr(self.path_curve), _ptr(self.curve_start), _ptr(self.curve_gear),
-                _ptr(self.robot_path), _ptr(self.curve_index), _ptr(self.cur_index), 0.1, 10, _ptr(nom_s), _ptr(ref_s),
-                _ptr(near), _ptr(solver_speed), _stream(dev)), 'rda_pre_process_paths')
+            if self.per_robot is None:
+                _cabi.check(self.lib.rda_pre_process_paths(
+                    B, T, _cabi.DYNAMICS[self.dynamics], self.dt, self.L, _ptr(state), _ptr(self.cur_vel),
+                    _ptr(ref_speed), *paths), 'rda_pre_process_paths')
+            else:
+                _cabi.check(self.lib.rda_pre_process_paths_per_robot(
+                    B, T, _ptr(self.per_robot['dynamics']), self.dt, _ptr(self.per_robot['wheelbase']), _ptr(state),
+                    _ptr(self.cur_vel), _ptr(ref_speed), *paths), 'rda_pre_process_paths_per_robot')
         self.cur_index = near
         if (shapes is None and world is None) or self.N == 0:
             A, b, kind, count = self._no_obstacles()
             time_varying = False
         elif avoid_fleet:
-            fleet = fleet_shapes_batch(state, self.cur_vel, self.body, self.dynamics)
+            fleet = fleet_shapes_batch(state, self.cur_vel, self.body, self.dynamics, self.per_robot)
             A, b, kind, count = convert_fleet_obstacles_batch(world, state, robot_world, fleet, self.N, T, self.E,
                                                               self.dt, time_varying, self.obstacle_order)
         elif world is not None:
@@ -455,6 +512,11 @@ class BatchedMPC:
     def advance(self, state):
         """One simulator step with the first control of the last solve (mpc.py:293-336), in place."""
         with torch.cuda.device(self.device):
+            if self.per_robot is not None:
+                _cabi.check(self.lib.rda_motion_predict_per_robot(
+                    self.batch, self.T, _ptr(self.per_robot['dynamics']), self.dt, _ptr(self.per_robot['wheelbase']),
+                    _ptr(self.cur_vel), _ptr(state), _stream(self.device)), 'rda_motion_predict_per_robot')
+                return state
             _cabi.check(self.lib.rda_motion_predict(self.batch, self.T, _cabi.DYNAMICS[self.dynamics], self.dt, self.L,
                                                     _ptr(self.cur_vel), _ptr(state), _stream(self.device)),
                         'rda_motion_predict')

@@ -242,6 +242,51 @@ def update_instance_table(table, dt, robots=None, validate=True, **values):
     return out
 
 
+def robot_body(car_tuple):
+    """(G, h, robot cone) of a car_tuple's body as the kernels take it: a polygon's rows in canonical counter-clockwise
+    order (canonical_polygon_rows), or the disc G = [[1,0],[0,1],[0,0]], h = (cx, cy, -r) of cone_type 'norm2'."""
+    G = np.asarray(car_tuple.G, float)
+    h = np.asarray(car_tuple.h, float).reshape(-1)
+    if car_tuple.cone_type == 'norm2':
+        # disc body (cone_cp_array(-mu, 'norm2'), :1034-1039) as ir-sim describes it: |y - (h0, h1)| <= -h2
+        if G.shape != (3, 2) or np.abs(G - np.array([[1.0, 0], [0, 1], [0, 0]])).max() > 1e-9 or not h[2] < 0:
+            raise NotImplementedError("norm2 robot: only the disc G = [[1,0],[0,1],[0,0]], h = (cx, cy, -r) is supported")
+        return G, h, _cabi.ROBOT_DISC
+    if car_tuple.cone_type == 'Rpositive':
+        G, h = canonical_polygon_rows(G, h)
+        return G, h, _cabi.ROBOT_POLYGON
+    raise ValueError(f'unknown robot cone type {car_tuple.cone_type!r}')
+
+
+def robot_class_table(car_tuples, cone_type, R):
+    """The rda_robot_class array of car_tuples (at most RDA_MAX_ROBOT_CLASSES) for a solver whose body has cone_type and
+    R canonical rows; raises ValueError naming the first class the kernels cannot take."""
+    K = len(car_tuples)
+    if K > _cabi.MAX_ROBOT_CLASSES:
+        raise ValueError(f'at most {_cabi.MAX_ROBOT_CLASSES} robot classes, got {K}')
+    arr = (_cabi.RobotClass * max(K, 1))()
+    for k, car in enumerate(car_tuples):
+        if car.cone_type != cone_type:
+            raise ValueError(f'robot class {k}: cone_type {car.cone_type!r} differs from the solver\'s {cone_type!r}')
+        G, h, _ = robot_body(car)
+        if G.shape[0] != R:
+            raise ValueError(f'robot class {k}: {G.shape[0]} canonical body rows, the solver has {R}')
+        if car.dynamics not in _cabi.DYNAMICS:
+            raise ValueError(f'robot class {k}: unknown dynamics {car.dynamics!r}')
+        L = float(car.wheelbase)
+        if not np.isfinite(L) or (car.dynamics == 'acker' and not L > 0):
+            raise ValueError(f'robot class {k}: wheelbase must be finite, and > 0 for acker (got {car.wheelbase})')
+        for key in ('max_speed', 'max_acce'):
+            try:
+                _host_instance_value(key, np.asarray(getattr(car, key), float).reshape(-1)[:2], 1)
+            except ValueError as e:
+                raise ValueError(f'robot class {k}: {e}') from None
+        arr[k].dynamics, arr[k].wheelbase = _cabi.DYNAMICS[car.dynamics], L
+        for j in range(R):
+            arr[k].G[2 * j], arr[k].G[2 * j + 1], arr[k].h[j] = G[j, 0], G[j, 1], h[j]
+    return arr
+
+
 class RDA_solver:
     def __init__(self, receding, car_tuple, max_edge_num=5, max_obs_num=5, iter_num=2, step_time=0.1,
                  iter_threshold=0.2, process_num=4, accelerated=True, time_print=True, batch=1,
@@ -270,18 +315,7 @@ class RDA_solver:
         self.batch = batch
         self.ws = kwargs.get('ws', 1)
         self.wu = kwargs.get('wu', 1)
-        G = np.asarray(car_tuple.G, float)
-        h = np.asarray(car_tuple.h, float).reshape(-1)
-        if car_tuple.cone_type == 'norm2':
-            # disc body (cone_cp_array(-mu, 'norm2'), :1034-1039) as ir-sim describes it: |y - (h0, h1)| <= -h2
-            if G.shape != (3, 2) or np.abs(G - np.array([[1.0, 0], [0, 1], [0, 0]])).max() > 1e-9 or not h[2] < 0:
-                raise NotImplementedError("norm2 robot: only the disc G = [[1,0],[0,1],[0,0]], h = (cx, cy, -r) is supported")
-            robot_cone = _cabi.ROBOT_DISC
-        elif car_tuple.cone_type == 'Rpositive':
-            G, h = canonical_polygon_rows(G, h)
-            robot_cone = _cabi.ROBOT_POLYGON
-        else:
-            raise ValueError(f'unknown robot cone type {car_tuple.cone_type!r}')
+        G, h, robot_cone = robot_body(car_tuple)
         R = G.shape[0]
         if R > _cabi.MAX_ROBOT_EDGE or self.max_edge_num > _cabi.MAX_EDGE:
             raise ValueError('at most 8 robot edges / obstacle edges are supported')
@@ -330,6 +364,9 @@ class RDA_solver:
         self._graphs = {}
         self._static = None
         self._inst = None           # the installed per-instance table [B, RDA_INST_PARAMS] (set_instance_parameters)
+        self._classes = None        # the installed robot classes (set_robot_classes): car_tuples
+        self._class_index = None    # their index [B] (int32 CUDA tensor)
+        self._class_limits = None   # max_speed, max_acce of each class slot [K + 1, 2] (float64 CUDA tensors)
 
     def __del__(self):
         try:
@@ -404,6 +441,109 @@ class RDA_solver:
         out['acce_bound'] = out.pop('max_acce')
         out['max_acce'] = (out['acce_bound'].double() / self.dt).float()
         return {k: v.clone() for k, v in out.items()}
+
+    # ------------------------------------------------------------------ robot classes
+    def set_robot_classes(self, car_tuples, robot_class):
+        """Give each instance the body, wheelbase, dynamics and limits of a robot class: car_tuples is a list of at most
+        16 car_tuples (G h cone_type wheelbase max_speed max_acce dynamics) with the constructor's cone_type and as many
+        canonical rows (canonical_polygon_rows) as its body; robot_class [B] picks instance b's class, as an array-like
+        or an integer CUDA tensor.  An index outside [0, len(car_tuples)) means the constructor's car_tuple.  Each
+        instance's max_speed / max_acce become those of its class through set_instance_parameters (gathered on the
+        device); a later set_instance_parameters still overrides them.  Raises ValueError naming the offending class.
+        A set-up call: the classes and their limits are uploaded before it returns (the host waits for that copy);
+        set_robot_class_index then moves robots between classes without host synchronisation."""
+        car_tuples = list(car_tuples)
+        arr = robot_class_table(car_tuples, self.car_tuple.cone_type, self._cfg.robot_edges)
+        K = len(car_tuples)
+        index = self._class_index_tensor(robot_class, K)
+        with torch.cuda.device(self.device):
+            rc = self.lib.rda_set_robot_classes(self._h, K, arr, self._stream())
+            if rc == _cabi.E_UNSUPPORTED:
+                raise ValueError('robot class body not accepted: its rows must describe a closed convex polygon '
+                                 '(or the disc of cone_type norm2)')
+            _cabi.check(rc, 'rda_set_robot_classes')
+        self._graphs.clear()        # captured launches carry the number of classes
+        self._classes = car_tuples
+        # max_speed / max_acce of each class slot [K + 1, 2] (slot K: the constructor's car_tuple), uploaded once here so
+        # that moving robots between classes gathers on the device only
+        cars = car_tuples + [self.car_tuple]
+        pair = lambda key: torch.tensor(np.array([np.asarray(getattr(c, key), float).reshape(-1)[:2] for c in cars]),
+                                        dtype=torch.float64, device=self.device)
+        self._class_limits = (pair('max_speed'), pair('max_acce'))
+        self._class_index = None
+        self._install_class_index(index, None)
+
+    def set_robot_class_index(self, robot_class, robots=None):
+        """Move instances to other classes of the installed set (set_robot_classes): robot_class [B] (or one index),
+        applied to the robots of the bool mask robots [B] (None: all).  The robots whose class changes get their new
+        class's max_speed / max_acce; the others keep their rows.  Without host synchronisation when robot_class and
+        robots are CUDA tensors; a captured graph sees the new index."""
+        if self._classes is None:
+            raise RuntimeError('set_robot_classes first')
+        index = self._class_index_tensor(robot_class)
+        if robots is not None:
+            robots = torch.as_tensor(robots, device=self.device)
+            if robots.dtype != torch.bool or robots.shape != (self.batch,):
+                raise ValueError(f'robots: expected a bool mask of shape ({self.batch},), got {robots.dtype} '
+                                 f'{tuple(robots.shape)}')
+            index = torch.where(robots, index, self._class_index).contiguous()
+        self._install_class_index(index, self._class_index)
+
+    def clear_robot_classes(self):
+        """Back to the constructor's body, wheelbase, dynamics and limits for every instance."""
+        if self._classes is not None and self._inst is not None:
+            self._apply_class_limits(torch.full((self.batch,), -1, dtype=torch.int32, device=self.device))
+        with torch.cuda.device(self.device):
+            _cabi.check(self.lib.rda_set_robot_class_index(self._h, None, self._stream()), 'rda_set_robot_class_index')
+            _cabi.check(self.lib.rda_set_robot_classes(self._h, 0, None, self._stream()), 'rda_set_robot_classes')
+        self._graphs.clear()
+        self._classes = self._class_index = None
+
+    def robot_class_index(self):
+        """The installed class index [B] (a copy; -1 for an index outside the classes), or None."""
+        return None if self._class_index is None else self._class_index.clone()
+
+    def class_slot(self, index=None):
+        """Slot of each instance in tables of K + 1 class rows [B] (int64, on the device): its class, or K for an index
+        outside the classes (the constructor's car_tuple)."""
+        index = self._class_index if index is None else index
+        K = len(self._classes)
+        return torch.where((index >= 0) & (index < K), index, torch.full_like(index, K)).long()
+
+    def _class_index_tensor(self, robot_class, K=None):
+        """robot_class as int32 [B] on the device, every value outside [0, K) made -1 before the narrowing (so that a
+        wide integer cannot wrap into a valid class)."""
+        B, K = self.batch, len(self._classes) if K is None else K
+        if isinstance(robot_class, torch.Tensor):
+            if robot_class.dim() not in (0, 1) or (robot_class.dim() == 1 and robot_class.shape != (B,)) \
+                    or robot_class.is_floating_point() or robot_class.dtype == torch.bool:
+                raise ValueError(f'robot_class: expected an integer tensor of shape ({B},), got {robot_class.dtype} '
+                                 f'{tuple(robot_class.shape)}')
+            x = robot_class.to(self.device).expand(B)
+            return torch.where((x >= 0) & (x < K), x, torch.full_like(x, -1)).to(torch.int32).contiguous()
+        a = np.asarray(robot_class)
+        if a.ndim == 0:
+            a = np.full(B, a)
+        if a.shape != (B,) or not np.issubdtype(a.dtype, np.integer):
+            raise ValueError(f'robot_class: expected integers of shape ({B},), got {a.dtype} {a.shape}')
+        a = np.where((a >= 0) & (a < K), a, -1).astype(np.int32)
+        return torch.as_tensor(a, device=self.device)
+
+    def _apply_class_limits(self, index, robots=None):
+        """max_speed / max_acce of each instance's class (the constructor's for an index outside the classes) into the
+        rows of the robots of mask robots (None: all) of the per-instance table, gathered on the device."""
+        slot = self.class_slot(index)
+        ms, ma = self._class_limits
+        self.set_instance_parameters(robots, max_speed=ms[slot], max_acce=ma[slot])
+
+    def _install_class_index(self, index, previous):
+        with torch.cuda.device(self.device):
+            _cabi.check(self.lib.rda_set_robot_class_index(self._h, C.c_void_p(index.data_ptr()), self._stream()),
+                        'rda_set_robot_class_index')
+        if previous is None:
+            self._graphs.clear()    # captured launches carry "no classes"; a later index is seen by a replay
+        self._class_index = index   # the copy into the handle's storage reads it on the current stream
+        self._apply_class_limits(index, None if previous is None else self.class_slot(index) != self.class_slot(previous))
 
     def get_adjust_parameter(self):
         t = _cabi.Tunables()
