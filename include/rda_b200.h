@@ -143,6 +143,25 @@ int rda_cold_start(rda_handle *h, void *cuda_stream);
  * residuals < iter_threshold, :594), enqueued on cuda_stream, no host synchronisation. */
 int rda_solve(rda_handle *h, const rda_inputs *in, const rda_outputs *out, int iter_num,
               float iter_threshold, void *cuda_stream);
+/* How close each plan comes to its obstacles: for every instance b, stage t = 0..T and obstacle slot o, the signed
+ * distance between the robot body placed at the pose s[b][:][t] and obstacle o as the solver receives it at stage t
+ * (copy t of obs_A / obs_b when obs_time_varying, else copy 0):
+ *     sd(P, Q) = max over unit w of ( min_{x in P} w.x - max_{y in Q} w.y ),
+ * the Euclidean distance of disjoint sets and minus the penetration depth of overlapping ones.  The pose is the true
+ * footprint of column t (position and heading of the same column), not the solver's pairing of the heading of column
+ * t with the position of column t+1.  The body is the instance's robot class's (rda_set_robot_class_index) or the
+ * handle's; polygon obstacles are the closed counter-clockwise rows the solve takes, discs rows [[1,0],[0,1],[0,0]] with
+ * b = (cx, cy, -r).  Slots o >= min(obs_count[b], N) (the padding copies) are +inf.
+ *   s [B][3][T+1] (e.g. rda_outputs.s_opt or rda_inputs.nom_s); dist [B][N][T+1] or NULL;
+ *   min_dist [B]: the minimum of the float32 values of instance b over its valid cells, +inf without one;
+ *   min_index [B]: the smallest o * (T+1) + t attaining it, -1 without a valid cell.  Cells of a non-finite pose
+ *   are written but do not take part in the minimum.
+ * Reads only the obstacle fields of `in`; touches no warm-start state, counter or rda_last_launch_count.  One kernel
+ * on cuda_stream, no host synchronisation, CUDA-graph capturable; results are bitwise reproducible.  RDA_E_ARG for a
+ * NULL h, in, s, min_dist or min_index, or NULL obstacle arrays when N > 0. */
+int rda_plan_clearance(rda_handle *h, const rda_inputs *in, const float *s /* [B][3][T+1] */,
+                       float *dist /* [B][N][T+1] or NULL */, float *min_dist /* [B] */,
+                       int32_t *min_index /* [B] */, void *cuda_stream);
 /* Single phases, for unit tests and profiling: begin (load nominal + obstacles), one su-QP
  * (su_prob_solve :692-700 + assign_state_parameter :436-460), one LamMuZ + multiplier update
  * (:702-741, :529-542, :639-690), and the output stage. */

@@ -61,7 +61,8 @@ EXPORTS = ['rda_create', 'rda_destroy', 'rda_set_tunables', 'rda_get_tunables', 
            'rda_pre_process_curves', 'rda_post_process_gear', 'rda_convert_world_obstacles',
            'rda_pre_process_paths', 'rda_post_process_paths', 'rda_fleet_shapes', 'rda_convert_fleet_obstacles',
            'rda_set_instance_params', 'rda_set_robot_classes', 'rda_set_robot_class_index',
-           'rda_pre_process_paths_per_robot', 'rda_motion_predict_per_robot', 'rda_fleet_shapes_per_robot']
+           'rda_pre_process_paths_per_robot', 'rda_motion_predict_per_robot', 'rda_fleet_shapes_per_robot',
+           'rda_plan_clearance']
 MAX_SHAPES = 64
 MAX_WORLD_SLOTS = 256
 
@@ -97,6 +98,7 @@ def load():
     lib.rda_get_buffer.argtypes = [vp, C.c_int, C.POINTER(vp), C.POINTER(C.c_size_t)]
     lib.rda_copy_buffer.argtypes = [vp, C.c_int, vp, C.c_int, vp]
     lib.rda_last_launch_count.argtypes = [vp]
+    lib.rda_plan_clearance.argtypes = [vp, C.POINTER(Inputs), vp, vp, vp, vp, vp]
     lib.rda_version.restype = C.c_char_p
     i, f = C.c_int, C.c_float
     lib.rda_pre_process.argtypes = [i, i, i, f, f, vp, vp, vp, vp, i, vp, f, i, vp, vp, vp, vp]

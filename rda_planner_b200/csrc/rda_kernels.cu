@@ -7,6 +7,7 @@
 //   k_finalize per instance: residuals, early-stop flag (:594-596)
 // No host synchronisation, no allocation, CUDA-graph capturable.
 #include <cuda_runtime.h>
+#include <limits.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -17,6 +18,7 @@
 #include "cell_lean.cuh"
 #include "cell_lean2.cuh"
 #include "cell_disc_robot.cuh"
+#include "plan_clearance.cuh"
 
 using namespace rda;
 
@@ -1231,6 +1233,59 @@ __global__ void k_fill(float* p, float v, size_t n) {
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) p[i] = v;
 }
 
+// (value, index) of two candidates: the smaller value, the smaller index among equal values (any reduction order gives
+// the same result)
+__device__ __forceinline__ void clear_min(float& v, int& i, float ov, int oi) {
+  if (ov < v || (ov == v && oi < i)) { v = ov; i = oi; }
+}
+
+// rda_plan_clearance: one CTA per instance b, its threads striding over the N * (T + 1) cells c = o * (T + 1) + t (t
+// fastest, the layout of dist), then the (value, index) minimum over each warp and over the CTA.  The body (the
+// instance's class's, or the handle's rbh) is staged once in shared memory.
+constexpr int CLEAR_THREADS = 128;
+template <int EC, int RC>
+__global__ void __launch_bounds__(CLEAR_THREADS) k_plan_clearance(const float* __restrict__ s, const float* __restrict__ obs_A,
+                                                                  const float* __restrict__ obs_b,
+                                                                  const int* __restrict__ obs_kind,
+                                                                  const int* __restrict__ obs_count, int tv, int T, int N,
+                                                                  int E, RobotGeom rbh, const int* __restrict__ cls,
+                                                                  int ncls, const RobotGeom* __restrict__ cls_rb,
+                                                                  float* __restrict__ dist, float* __restrict__ min_dist,
+                                                                  int* __restrict__ min_index) {
+  __shared__ RobotGeom body;
+  __shared__ float wv[CLEAR_THREADS / 32];
+  __shared__ int wi[CLEAR_THREADS / 32];
+  const int b = blockIdx.x;
+  if (threadIdx.x == 0) body = cls ? cls_rb[class_slot(cls, ncls, b)] : rbh;
+  __syncthreads();
+  const int T1 = T + 1, cells = N * T1;
+  const int valid = N > 0 ? min(max(obs_count[b], 0), N) : 0;
+  const size_t Tc = tv ? T1 : 1;
+  const float* sb = s + (size_t)b * 3 * T1;
+  float best = INFINITY;
+  int bi = INT_MAX;
+  for (int c = threadIdx.x; c < cells; c += CLEAR_THREADS) {
+    const int o = c / T1, t = c - o * T1;
+    float v = INFINITY;
+    if (o < valid) {
+      const size_t copy = ((size_t)b * N + o) * Tc + (tv ? t : 0);
+      v = (float)plan_clearance_cell<EC, RC>(body, obs_kind[(size_t)b * N + o], E, obs_A + copy * E * 2, obs_b + copy * E,
+                                             sb[t], sb[T1 + t], sb[2 * T1 + t]);
+      clear_min(best, bi, v, c);
+    }
+    if (dist) dist[(size_t)b * cells + c] = v;
+  }
+  for (int off = 16; off > 0; off >>= 1)
+    clear_min(best, bi, __shfl_xor_sync(0xffffffffu, best, off), __shfl_xor_sync(0xffffffffu, bi, off));
+  if ((threadIdx.x & 31) == 0) { wv[threadIdx.x >> 5] = best; wi[threadIdx.x >> 5] = bi; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < CLEAR_THREADS / 32; ++w) clear_min(best, bi, wv[w], wi[w]);
+    min_dist[b] = best;
+    min_index[b] = bi == INT_MAX ? -1 : bi;
+  }
+}
+
 // pointers of the sub-batch [b0, b0 + nb) (part selects its list counters)
 DevPtrs dev_ptrs(const rda_handle* h, int b0, int nb, int part) {
   DevPtrs d;
@@ -1749,6 +1804,19 @@ int rda_copy_buffer(rda_handle* h, int id, void* user, int to_handle, void* stre
   if (!user) return RDA_E_ARG;
   RDA_CUDA(cudaMemcpyAsync(to_handle ? p : user, to_handle ? user : p, n * 4, cudaMemcpyDeviceToDevice,
                            (cudaStream_t)stream));
+  return 0;
+}
+
+int rda_plan_clearance(rda_handle* h, const rda_inputs* in, const float* s, float* dist, float* min_dist,
+                       int32_t* min_index, void* stream) {
+  if (!h || !in || !s || !min_dist || !min_index) return RDA_E_ARG;
+  if (h->N > 0 && (!in->obs_A || !in->obs_b || !in->obs_kind || !in->obs_count)) return RDA_E_ARG;
+  const int* cls = h->cls_on && h->ncls > 0 ? h->cls_idx : nullptr;
+  auto k = h->E <= 4 && h->R <= 4 ? k_plan_clearance<4, 4> : k_plan_clearance<8, 8>;
+  k<<<h->B, CLEAR_THREADS, 0, (cudaStream_t)stream>>>(s, in->obs_A, in->obs_b, in->obs_kind, in->obs_count,
+                                                     in->obs_time_varying, h->T, h->N, h->E, h->rb, cls, h->ncls,
+                                                     h->cls_rb, dist, min_dist, min_index);
+  RDA_CUDA(cudaGetLastError());
   return 0;
 }
 

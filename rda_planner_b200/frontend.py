@@ -437,14 +437,16 @@ class BatchedMPC:
         return self._empty
 
     def control(self, state, ref_speed=5.0, shapes=None, time_varying=False, world=None, robot_world=None,
-                avoid_fleet=False):
+                avoid_fleet=False, clearance=False):
         """state [B,3] (CUDA tensor or array), ref_speed scalar or [B], shapes: dict from
         pack_shapes / shapes_to_device (None: free space).  Instead of shapes, world: dict from
         pack_worlds / shapes_to_device, obstacle maps shared by the robots, with robot_world [B] the map of
         each robot (may be omitted with a single map).  avoid_fleet: every robot also sees the other robots of its map
         (without world: all robots, in an empty map) as moving obstacles; not with shapes.  Returns (u0 [B,2], info)
         where info holds the solver's batched outputs plus 'arrive', 'nom_s', 'ref_s', 'cur_index', 'curve_index'.
-        No host sync."""
+        clearance: info also holds 'clearance' [B] and 'clearance_index' [B] of the plan just solved
+        (RDA_solver.plan_clearance: the smallest signed distance between a robot's planned footprints and the obstacles
+        it was given, negative inside one, and where it occurs).  No host sync."""
         dev, B, T = self.device, self.batch, self.T
         if avoid_fleet:
             if shapes is not None:
@@ -507,6 +509,9 @@ class BatchedMPC:
                                                         _ptr(self.arrive), _stream(dev)), 'rda_post_process_paths')
         info = dict(out)
         info.update(arrive=self.arrive, nom_s=nom_s, ref_s=ref_s, cur_index=near, curve_index=self.curve_index)
+        if clearance:
+            c = self.rda.plan_clearance()
+            info.update(clearance=c['min'], clearance_index=c['index'])
         return out['u'][:, :, 0], info
 
     def advance(self, state):

@@ -359,6 +359,7 @@ class RDA_solver:
             'iters': torch.empty(B, dtype=torch.int32, device=dev),
         }
         self._keep = None
+        self._keep_tv = 0
         self.obstacle_num = 0
         self.use_graph = bool(graph)
         self._graphs = {}
@@ -613,6 +614,7 @@ class RDA_solver:
             setattr(inp, k, t[k].data_ptr() if k in t else None)
         inp.obs_time_varying = int(bool(time_varying))
         self._keep = t          # the kernels read these buffers asynchronously
+        self._keep_tv = inp.obs_time_varying
         return inp
 
     def _outputs(self):
@@ -682,6 +684,41 @@ class RDA_solver:
 
     def launch_count(self):
         return self.lib.rda_last_launch_count(self._h)
+
+    def plan_clearance(self, s=None, per_cell=False):
+        """How close each plan comes to its obstacles (rda_plan_clearance): the signed distance between the robot body
+        (its class's, or the constructor's) placed at every pose s[b, :, t] and every obstacle the last solve (or begin)
+        received, at that obstacle's stage-t copy; negative where the body overlaps the obstacle (minus the penetration
+        depth).  The pose is the true footprint of column t: position and heading of the same column.  s: CUDA tensor
+        or array-like [B, 3, T+1]; default the last solve's s (e.g. pass nom_s, or the current state repeated, for a
+        check at the current pose).  Returns a dict of CUDA tensors: 'min' [B] float32 (the smallest distance of the
+        instance, +inf without obstacles) and 'index' [B] int32 (the smallest o * (T+1) + t attaining it, -1 without
+        obstacles), plus 'map' [B, N, T+1] (padding slots +inf) with per_cell.  Nothing the solver holds changes; no
+        host synchronisation.  Raises before the first solve."""
+        if self._keep is None:
+            raise RuntimeError('plan_clearance needs the obstacles of a solve: call a solve (or begin) first')
+        B, T, N, dev = self.batch, self.T, self.max_obs_num, self.device
+        if s is None:
+            s = self._out['s']
+        else:
+            s = _as_cuda_f32(s, dev)
+            if tuple(s.shape) != (B, 3, T + 1):
+                raise ValueError(f's: expected shape ({B}, 3, {T + 1}), got {tuple(s.shape)}')
+        out = {'min': torch.empty(B, dtype=torch.float32, device=dev),
+               'index': torch.empty(B, dtype=torch.int32, device=dev)}
+        if per_cell:
+            out['map'] = torch.empty((B, N, T + 1), dtype=torch.float32, device=dev)
+        inp = _cabi.Inputs()
+        for k in ('obs_A', 'obs_b', 'obs_kind', 'obs_count'):
+            setattr(inp, k, self._keep[k].data_ptr() if k in self._keep else None)
+        inp.obs_time_varying = self._keep_tv
+        with torch.cuda.device(dev):
+            _cabi.check(self.lib.rda_plan_clearance(self._h, C.byref(inp), C.c_void_p(s.data_ptr()),
+                                                    C.c_void_p(out['map'].data_ptr()) if per_cell else None,
+                                                    C.c_void_p(out['min'].data_ptr()),
+                                                    C.c_void_p(out['index'].data_ptr()), self._stream()),
+                        'rda_plan_clearance')
+        return out
 
     def _solve_static(self, nom_s, nom_u, ref, ref_speed, A, b, kind, count, tv):
         """graph=True, single instance: inputs are staged into persistent device buffers (one pinned host block, one
