@@ -285,6 +285,36 @@ int rda_convert_fleet_obstacles(int B, int W, int N, int T, int E, float dt, int
                                 float *obs_A, float *obs_b, int32_t *obs_kind, int32_t *obs_count,
                                 void *cuda_stream);
 
+/* A fleet that avoids each other's PLANS: every map-mate is a time-varying obstacle that follows the controls its last
+ * solve kept (cur_vel [B][2][T]) instead of moving at the constant velocity of the first one.  In the reference's terms
+ * each mate is an rdaobs whose A and b are lists of T+1 arrays (rda_solver.py:501-526), the rows of its body at its
+ * predicted pose of each stage.
+ * rda_fleet_plan_shapes writes what rda_fleet_shapes writes (bit for bit) and plan_xy [B][T+1][RDA_MAX_EDGE][2]
+ * (16-byte aligned): robot m's body placed at q_m(t), with q_m(0) = state[m] and, for t = 0..T-1,
+ * q_m(t+1) = motion_predict(q_m(t), cur_vel[m][:, c]), c = min(t + 1, T - 1), in double (column 0 is the control
+ * rda_motion_predict has just applied, so the rest of the plan starts at column 1; the last column is held).  Stage 0 is
+ * bit for bit the shape_xy of the same robot.  The dynamics, wheelbase and body are the scalars (checked as for
+ * rda_fleet_shapes), or per robot when dynamics_b int32 [B], wheelbase_b float32 [B], body_xy_b float32
+ * [B][RDA_MAX_EDGE][2] or body_radius_b float32 [B] are given (device; NULL: the scalar; values the caller's to check).
+ * rda_convert_fleet_plan_obstacles is rda_convert_fleet_obstacles, the same list, keys (from the stage-0 shapes), order,
+ * padding, obs_kind and obs_count, except that the stage-t copy of a mate's slot is the rows of its plan_xy[t] shape
+ * standing still (fleet_plan_xy: rda_fleet_plan_shapes' plan_xy).  World shapes keep their constant-velocity rows.  The
+ * prediction is a trajectory, so time_varying must be non-zero (RDA_E_ARG otherwise).  Neither call allocates, syncs
+ * the host or breaks graph capture.                                                                              */
+int rda_fleet_plan_shapes(int B, int T, int dynamics, float dt, float wheelbase, int body_kind, int body_nv,
+                          const float *body_xy, float body_radius, const int32_t *dynamics_b, const float *wheelbase_b,
+                          const float *body_xy_b, const float *body_radius_b, const float *state, const float *cur_vel,
+                          int32_t *shape_kind, int32_t *shape_nv, float *shape_xy, float *shape_radius,
+                          float *shape_vel, float *plan_xy, void *cuda_stream);
+int rda_convert_fleet_plan_obstacles(int B, int W, int N, int T, int E, float dt, int time_varying, int order,
+                                     const float *state, const int32_t *world_start, const int32_t *robot_world,
+                                     const int32_t *shape_kind, const int32_t *shape_nv, const float *shape_xy,
+                                     const float *shape_radius, const float *shape_vel, const int32_t *fleet_start,
+                                     const int32_t *fleet_robot, const int32_t *fleet_kind, const int32_t *fleet_nv,
+                                     const float *fleet_xy, const float *fleet_radius, const float *fleet_vel,
+                                     const float *fleet_plan_xy, float *obs_A, float *obs_b, int32_t *obs_kind,
+                                     int32_t *obs_count, void *cuda_stream);
+
 /* Arrive rule of MPC.control (mpc.py:170-185, single gear): instances whose near_index >=
  * P - goal_index_threshold get u_opt = 0 and arrive = 1; cur_vel (may be NULL) receives the
  * controls kept as the next step's nominal (mpc.py:186).  u_opt, cur_vel [B][2][T].        */

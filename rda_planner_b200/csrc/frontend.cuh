@@ -232,15 +232,10 @@ RDA_HD void obstacle_rows(int kind, int nv, const float* xy, double radius, doub
   }
 }
 
-// A robot of a fleet as one raw shape for its map-mates: the body (body frame: polygon vertices body_xy [nv][2],
-// counter-clockwise, or the disc centre body_xy[0..1] and body_radius) placed at the pose `state` (p + R(theta) v),
-// moving with the world-frame velocity of its control (v0, v1) as motion_predict moves it: v0 (cos, sin) of the
-// heading for acker / diff, of the control angle v1 for omni (mpc.py:293-336).  Entries of xy beyond the shape's own
-// are zero, as the host packing leaves them.
-RDA_HD void fleet_shape(int dynamics, int body_kind, int body_nv, const float* body_xy, float body_radius,
-                        const float* state, double v0, double v1, int* kind, int* nv, float* xy, float* radius,
-                        float* vel) {
-  const double px = state[0], py = state[1], th = state[2];
+// The body (body frame: polygon vertices body_xy [nv][2], counter-clockwise, or the disc centre body_xy[0..1]) placed
+// at the pose (px, py, th): p + R(th) v in double, rounded to float32.  Entries of xy beyond the shape's own are zero,
+// as the host packing leaves them.
+RDA_HD void place_body(int body_kind, int body_nv, const float* body_xy, double px, double py, double th, float* xy) {
   const double c = cos(th), s = sin(th);
   const int n = body_kind == RDA_OBS_CIRCLE ? 1 : body_nv;
   for (int i = 0; i < RDA_MAX_EDGE; ++i) {
@@ -252,12 +247,49 @@ RDA_HD void fleet_shape(int dynamics, int body_kind, int body_nv, const float* b
       xy[2 * i] = 0.f; xy[2 * i + 1] = 0.f;
     }
   }
+}
+
+// A robot of a fleet as one raw shape for its map-mates: the body (body_radius: the disc's) placed at the pose `state`
+// (place_body), moving with the world-frame velocity of its control (v0, v1) as motion_predict moves it: v0 (cos, sin)
+// of the heading for acker / diff, of the control angle v1 for omni (mpc.py:293-336).
+RDA_HD void fleet_shape(int dynamics, int body_kind, int body_nv, const float* body_xy, float body_radius,
+                        const float* state, double v0, double v1, int* kind, int* nv, float* xy, float* radius,
+                        float* vel) {
+  const double th = state[2];
+  place_body(body_kind, body_nv, body_xy, state[0], state[1], th, xy);
   *kind = body_kind;
   *nv = body_kind == RDA_OBS_CIRCLE ? 0 : body_nv;
   *radius = body_kind == RDA_OBS_CIRCLE ? body_radius : 0.f;
   const double dir = dynamics == RDA_DYN_OMNI ? v1 : th;
   vel[0] = (float)(v0 * cos(dir));
   vel[1] = (float)(v0 * sin(dir));
+}
+
+// A robot of a fleet predicted along its plan, as the stage-t shapes of a time-varying obstacle for its map-mates:
+// q(0) = state, q(t+1) = motion_predict(q(t), u[:, c]) with c = min(t + 1, T - 1) for t = 0..T-1, in double (column 0
+// of u [2][T] (row stride T) is the control the robot has just applied, so its plan goes on from column 1 and holds its
+// last column); stage t is the body placed at q(t) (place_body), written to plan_xy [T+1][RDA_MAX_EDGE][2].  Stage 0 is
+// bit for bit the xy of fleet_shape at the same state.  On the device plan_xy must be 16-byte aligned: each stage is
+// stored as four 16-byte vectors.
+RDA_HD void fleet_plan(int dynamics, double dt, double L, int body_kind, int body_nv, const float* body_xy,
+                       const float* state, const float* u, int T, float* plan_xy) {
+  double q[3] = {state[0], state[1], state[2]};
+  for (int t = 0;; ++t) {
+    float xy[2 * RDA_MAX_EDGE];
+    place_body(body_kind, body_nv, body_xy, q[0], q[1], q[2], xy);
+    float* out = plan_xy + (size_t)t * 2 * RDA_MAX_EDGE;
+#ifdef __CUDA_ARCH__
+    for (int i = 0; i < 2 * RDA_MAX_EDGE; i += 4)
+      *reinterpret_cast<float4*>(out + i) = make_float4(xy[i], xy[i + 1], xy[i + 2], xy[i + 3]);
+#else
+    for (int i = 0; i < 2 * RDA_MAX_EDGE; ++i) out[i] = xy[i];
+#endif
+    if (t == T) break;
+    const int c = t + 1 < T ? t + 1 : T - 1;
+    double nxt[3];
+    motion_predict(dynamics, dt, L, q, u[c], u[T + c], nxt);
+    q[0] = nxt[0]; q[1] = nxt[1]; q[2] = nxt[2];
+  }
 }
 
 // the order of the stable sort by key: ties go to the lower list index

@@ -129,13 +129,16 @@ __device__ __forceinline__ size_t list_entry(const ShapeList& L, int i, const in
   return (size_t)(m < 0 ? 0 : (m >= B ? B - 1 : m));   // a malformed list never reads outside the fleet
 }
 
+// kPlan: map-mates are read along their plans, fleet_plan_xy [B][T+1][RDA_MAX_EDGE][2] (time-varying output only);
+// the variant without plans never reads it, and compiles to the code it had before plans existed.
+template <bool kPlan>
 __global__ void __launch_bounds__(kWorldTile)
 k_convert_world_obstacles(int B, int W, int N, int T, int E, float dt, int time_varying, int order, const float* state,
                           const int* world_start, const int* robot_world, const int* shape_kind, const int* shape_nv,
                           const float* shape_xy, const float* shape_radius, const float* shape_vel,
                           const int* fleet_start, const int* fleet_robot, const int* fleet_kind, const int* fleet_nv,
-                          const float* fleet_xy, const float* fleet_radius, const float* fleet_vel, float* obs_A,
-                          float* obs_b, int* obs_kind, int* obs_count) {
+                          const float* fleet_xy, const float* fleet_radius, const float* fleet_vel,
+                          const float* fleet_plan_xy, float* obs_A, float* obs_b, int* obs_kind, int* obs_count) {
   // dynamic shared memory (order != 0): kept keys [2][N], candidate keys [2][tile], kept indices [2][N],
   // candidate indices [2][tile]; the kept list is double-buffered, candidates are gathered then sorted
   extern __shared__ double sh[];
@@ -230,19 +233,31 @@ k_convert_world_obstacles(int B, int W, int N, int T, int E, float dt, int time_
     const size_t s = list_entry(L, src, fleet_robot, b, B, &mate);
     const int kind = (mate ? fleet_kind : shape_kind)[s];
     if (t == 0) obs_kind[(size_t)b * N + n] = kind;
-    const float* vel = (mate ? fleet_vel : shape_vel) + 2 * s;
-    obstacle_rows(kind, (mate ? fleet_nv : shape_nv)[s], (mate ? fleet_xy : shape_xy) + s * RDA_MAX_EDGE * 2,
-                  (mate ? fleet_radius : shape_radius)[s], vel[0], vel[1], t, (double)dt, E, A, bb);
+    const float* xy = (mate ? fleet_xy : shape_xy) + s * RDA_MAX_EDGE * 2;
+    double vx = 0.0, vy = 0.0;
+    if (kPlan && mate) {                               // a map-mate along its plan: its stage-t shape, standing
+      xy = fleet_plan_xy + (s * (T + 1) + t) * RDA_MAX_EDGE * 2;
+    } else {
+      const float* vel = (mate ? fleet_vel : shape_vel) + 2 * s;
+      vx = vel[0]; vy = vel[1];
+    }
+    obstacle_rows(kind, (mate ? fleet_nv : shape_nv)[s], xy, (mate ? fleet_radius : shape_radius)[s], vx, vy, t,
+                  (double)dt, E, A, bb);
   }
 }
 
 // Each robot of a fleet as a raw shape for its map-mates (fleet_shape), one thread per robot: its body at its pose,
 // moving with the first control of cur_vel, the one rda_motion_predict moved it with.  dyn_b [B], body_xy_b [B][8][2] and
 // body_radius_b [B]: each robot's own dynamics and body (robot classes), or NULL: the scalars / the one body for every robot.
+// kPlan: also each robot's body along its plan, plan_xy [B][T+1][RDA_MAX_EDGE][2] (16-byte aligned; fleet_plan, serial
+// over T in the robot's thread), with time step dt and wheelbase L, or L_b [B] per robot.  The variant without plans
+// never reads them, and compiles to the code it had before plans existed.
+template <bool kPlan>
 __global__ void k_fleet_shapes(int B, int T, int dynamics, int body_kind, int body_nv, const float* body_xy,
                                float body_radius, const int* dyn_b, const float* body_xy_b, const float* body_radius_b,
                                const float* state, const float* cur_vel, int* shape_kind,
-                               int* shape_nv, float* shape_xy, float* shape_radius, float* shape_vel) {
+                               int* shape_nv, float* shape_xy, float* shape_radius, float* shape_vel, float dt, float L,
+                               const float* L_b, float* plan_xy) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
   const float* u = cur_vel + (size_t)b * 2 * T;
@@ -252,6 +267,10 @@ __global__ void k_fleet_shapes(int B, int T, int dynamics, int body_kind, int bo
   fleet_shape(dynamics, body_kind, body_nv, body_xy, body_radius, state + 3 * (size_t)b, (double)u[0], (double)u[T],
               shape_kind + b, shape_nv + b, shape_xy + (size_t)b * RDA_MAX_EDGE * 2, shape_radius + b,
               shape_vel + 2 * (size_t)b);
+  if (!kPlan) return;
+  if (L_b) L = L_b[b];
+  fleet_plan(dynamics, (double)dt, (double)L, body_kind, body_nv, body_xy, state + 3 * (size_t)b, u, T,
+             plan_xy + (size_t)b * (T + 1) * RDA_MAX_EDGE * 2);
 }
 
 // End-of-curve and arrive rules of MPC.control (mpc.py:166-185) on each robot's own curve and path, one thread per
@@ -297,25 +316,27 @@ __global__ void k_motion_predict(int B, int T, int dynamics, float dt, float L, 
 }
 
 // Argument checks and launch of k_convert_world_obstacles.  Without `fleet` the fleet pointers are NULL and each robot
-// chooses from its world's shapes only.
+// chooses from its world's shapes only; fleet_plan_xy (fleet only, time-varying output only) may be NULL.
 int launch_world_obstacles(bool fleet, int B, int W, int N, int T, int E, float dt, int time_varying, int order,
                            const float* state, const int32_t* world_start, const int32_t* robot_world,
                            const int32_t* shape_kind, const int32_t* shape_nv, const float* shape_xy,
                            const float* shape_radius, const float* shape_vel, const int32_t* fleet_start,
                            const int32_t* fleet_robot, const int32_t* fleet_kind, const int32_t* fleet_nv,
-                           const float* fleet_xy, const float* fleet_radius, const float* fleet_vel, float* obs_A,
-                           float* obs_b, int32_t* obs_kind, int32_t* obs_count, cudaStream_t stream) {
+                           const float* fleet_xy, const float* fleet_radius, const float* fleet_vel,
+                           const float* fleet_plan_xy, float* obs_A, float* obs_b, int32_t* obs_kind,
+                           int32_t* obs_count, cudaStream_t stream) {
   if (B < 1 || W < 1 || N < 1 || T < 1) return RDA_E_ARG;
   if (N > RDA_MAX_WORLD_SLOTS || E < 3 || E > RDA_MAX_EDGE) return RDA_E_UNSUPPORTED;
   if (!world_start || !shape_kind || !shape_nv || !shape_xy || !shape_radius || !shape_vel) return RDA_E_ARG;
   if (!obs_A || !obs_b || !obs_kind || !obs_count || (order && !state)) return RDA_E_ARG;
   if (fleet && (!fleet_start || !fleet_robot || !fleet_kind || !fleet_nv || !fleet_xy || !fleet_radius || !fleet_vel))
     return RDA_E_ARG;
+  if (fleet_plan_xy && (!fleet || !time_varying)) return RDA_E_ARG;
   const size_t smem = order ? (size_t)(2 * N + 2 * kWorldTile) * (sizeof(double) + sizeof(int)) : 0;
-  k_convert_world_obstacles<<<B, kWorldTile, smem, stream>>>(
+  (fleet_plan_xy ? k_convert_world_obstacles<true> : k_convert_world_obstacles<false>)<<<B, kWorldTile, smem, stream>>>(
       B, W, N, T, E, dt, time_varying, order, state, world_start, robot_world, shape_kind, shape_nv, shape_xy,
       shape_radius, shape_vel, fleet_start, fleet_robot, fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel,
-      obs_A, obs_b, obs_kind, obs_count);
+      fleet_plan_xy, obs_A, obs_b, obs_kind, obs_count);
   RDA_CUDA(cudaGetLastError());
   return 0;
 }
@@ -424,7 +445,7 @@ int rda_convert_world_obstacles(int B, int W, int N, int T, int E, float dt, int
                                 int32_t* obs_kind, int32_t* obs_count, void* stream) {
   return launch_world_obstacles(false, B, W, N, T, E, dt, time_varying, order, state, world_start, robot_world,
                                 shape_kind, shape_nv, shape_xy, shape_radius, shape_vel, nullptr, nullptr, nullptr,
-                                nullptr, nullptr, nullptr, nullptr, obs_A, obs_b, obs_kind, obs_count,
+                                nullptr, nullptr, nullptr, nullptr, nullptr, obs_A, obs_b, obs_kind, obs_count,
                                 (cudaStream_t)stream);
 }
 
@@ -439,9 +460,10 @@ int rda_fleet_shapes(int B, int T, int dynamics, int body_kind, int body_nv, con
   }
   if (!body_xy || !state || !cur_vel || !shape_kind || !shape_nv || !shape_xy || !shape_radius || !shape_vel)
     return RDA_E_ARG;
-  k_fleet_shapes<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(B, T, dynamics, body_kind, body_nv, body_xy,
+  k_fleet_shapes<false><<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(B, T, dynamics, body_kind, body_nv, body_xy,
                                                                      body_radius, nullptr, nullptr, nullptr, state, cur_vel,
-                                                                     shape_kind, shape_nv, shape_xy, shape_radius, shape_vel);
+                                                                     shape_kind, shape_nv, shape_xy, shape_radius, shape_vel,
+                                                                     0.f, 0.f, nullptr, nullptr);
   RDA_CUDA(cudaGetLastError());
   return 0;
 }
@@ -458,9 +480,10 @@ int rda_fleet_shapes_per_robot(int B, int T, const int32_t* dynamics, int body_k
   if (!body_xy || !body_radius || !state || !cur_vel || !shape_kind || !shape_nv || !shape_xy || !shape_radius ||
       !shape_vel)
     return RDA_E_ARG;
-  k_fleet_shapes<<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(B, T, 0, body_kind, body_nv, nullptr, 0.f, dynamics,
+  k_fleet_shapes<false><<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(B, T, 0, body_kind, body_nv, nullptr, 0.f, dynamics,
                                                                      body_xy, body_radius, state, cur_vel, shape_kind,
-                                                                     shape_nv, shape_xy, shape_radius, shape_vel);
+                                                                     shape_nv, shape_xy, shape_radius, shape_vel, 0.f, 0.f,
+                                                                     nullptr, nullptr);
   RDA_CUDA(cudaGetLastError());
   return 0;
 }
@@ -474,8 +497,44 @@ int rda_convert_fleet_obstacles(int B, int W, int N, int T, int E, float dt, int
                                 float* obs_b, int32_t* obs_kind, int32_t* obs_count, void* stream) {
   return launch_world_obstacles(true, B, W, N, T, E, dt, time_varying, order, state, world_start, robot_world,
                                 shape_kind, shape_nv, shape_xy, shape_radius, shape_vel, fleet_start, fleet_robot,
-                                fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel, obs_A, obs_b, obs_kind,
-                                obs_count, (cudaStream_t)stream);
+                                fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel, nullptr, obs_A, obs_b,
+                                obs_kind, obs_count, (cudaStream_t)stream);
+}
+
+int rda_fleet_plan_shapes(int B, int T, int dynamics, float dt, float wheelbase, int body_kind, int body_nv,
+                          const float* body_xy, float body_radius, const int32_t* dynamics_b, const float* wheelbase_b,
+                          const float* body_xy_b, const float* body_radius_b, const float* state, const float* cur_vel,
+                          int32_t* shape_kind, int32_t* shape_nv, float* shape_xy, float* shape_radius,
+                          float* shape_vel, float* plan_xy, void* stream) {
+  if (B < 1 || T < 1 || (!dynamics_b && (dynamics < 0 || dynamics > 2))) return RDA_E_ARG;
+  if (body_kind == RDA_OBS_POLYGON) {
+    if (body_nv < 3 || body_nv > RDA_MAX_EDGE) return RDA_E_UNSUPPORTED;
+  } else if (body_kind != RDA_OBS_CIRCLE || (!body_radius_b && !(body_radius > 0.f))) {
+    return RDA_E_ARG;
+  }
+  if ((!body_xy && !body_xy_b) || !state || !cur_vel || !shape_kind || !shape_nv || !shape_xy || !shape_radius ||
+      !shape_vel || !plan_xy || ((uintptr_t)plan_xy & 15))
+    return RDA_E_ARG;
+  k_fleet_shapes<true><<<(B + 127) / 128, 128, 0, (cudaStream_t)stream>>>(
+      B, T, dynamics, body_kind, body_nv, body_xy, body_radius, dynamics_b, body_xy_b, body_radius_b, state, cur_vel,
+      shape_kind, shape_nv, shape_xy, shape_radius, shape_vel, dt, wheelbase, wheelbase_b, plan_xy);
+  RDA_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int rda_convert_fleet_plan_obstacles(int B, int W, int N, int T, int E, float dt, int time_varying, int order,
+                                     const float* state, const int32_t* world_start, const int32_t* robot_world,
+                                     const int32_t* shape_kind, const int32_t* shape_nv, const float* shape_xy,
+                                     const float* shape_radius, const float* shape_vel, const int32_t* fleet_start,
+                                     const int32_t* fleet_robot, const int32_t* fleet_kind, const int32_t* fleet_nv,
+                                     const float* fleet_xy, const float* fleet_radius, const float* fleet_vel,
+                                     const float* fleet_plan_xy, float* obs_A, float* obs_b, int32_t* obs_kind,
+                                     int32_t* obs_count, void* stream) {
+  if (!fleet_plan_xy) return RDA_E_ARG;
+  return launch_world_obstacles(true, B, W, N, T, E, dt, time_varying, order, state, world_start, robot_world,
+                                shape_kind, shape_nv, shape_xy, shape_radius, shape_vel, fleet_start, fleet_robot,
+                                fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel, fleet_plan_xy, obs_A, obs_b,
+                                obs_kind, obs_count, (cudaStream_t)stream);
 }
 
 int rda_post_process(int B, int T, int P, int goal_index_threshold, const int32_t* near_index, float* u_opt,

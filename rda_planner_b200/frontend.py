@@ -8,6 +8,7 @@
                            robot's N nearest shapes of its world
   fleet_shapes_batch, convert_fleet_obstacles_batch
                            the same with the other robots of each world as moving obstacles
+  fleet_plan_shapes_batch  the robots along their last plans, for convert_fleet_obstacles_batch(plan=True)
   pack_paths               a set of reference paths cut into single-gear curves (split_path, mpc.py:232-249),
                            in the layout the device reads
   BatchedMPC               MPC.control for B robots, on one reference path or each on its own path of a
@@ -259,6 +260,30 @@ def fleet_shapes_batch(state, cur_vel, body, dynamics, per_robot=None):
     return out
 
 
+def fleet_plan_shapes_batch(state, cur_vel, body, dynamics, dt, wheelbase, per_robot=None):
+    """fleet_shapes_batch (the same entries, bit for bit) plus 'plan_xy' [B,T+1,8,2]: each robot's body along its plan,
+    at q(0) = state and q(t+1) = the model step from q(t) with cur_vel[:, :, min(t + 1, T - 1)] (column 0 is the control
+    it has just applied).  per_robot: None, or a dict as for fleet_shapes_batch with also 'wheelbase' float32 [B]."""
+    lib = _cabi.load()
+    dev = state.device
+    B, T = state.shape[0], cur_vel.shape[2]
+    out = {'kind': torch.empty(B, dtype=torch.int32, device=dev), 'nv': torch.empty(B, dtype=torch.int32, device=dev),
+           'xy': torch.empty((B, _cabi.MAX_EDGE, 2), dtype=torch.float32, device=dev),
+           'radius': torch.empty(B, dtype=torch.float32, device=dev),
+           'vel': torch.empty((B, 2), dtype=torch.float32, device=dev),
+           'plan_xy': torch.empty((B, T + 1, _cabi.MAX_EDGE, 2), dtype=torch.float32, device=dev)}
+    pr = per_robot or {}
+    with torch.cuda.device(dev):
+        _cabi.check(lib.rda_fleet_plan_shapes(B, T, _cabi.DYNAMICS[dynamics], dt, wheelbase, body['kind'], body['nv'],
+                                              _ptr(body['xy']), body['radius'], _ptr(pr.get('dynamics')),
+                                              _ptr(pr.get('wheelbase')), _ptr(pr.get('xy')), _ptr(pr.get('radius')),
+                                              _ptr(state), _ptr(cur_vel), _ptr(out['kind']), _ptr(out['nv']),
+                                              _ptr(out['xy']), _ptr(out['radius']), _ptr(out['vel']),
+                                              _ptr(out['plan_xy']), _stream(dev)),
+                    'rda_fleet_plan_shapes')
+    return out
+
+
 def fleet_csr(robot_world, W):
     """robot_world [B] int32 CUDA tensor -> (start [W+1], robots [B]) int32: the robots of world w are
     robots[start[w]:start[w+1]], in ascending order; robots outside [0, W) are in no world.  On the device, without a
@@ -269,11 +294,16 @@ def fleet_csr(robot_world, W):
     return start, robots.to(torch.int32)
 
 
-def convert_fleet_obstacles_batch(world, state, robot_world, fleet, N, T, E, dt, time_varying=False, order=True):
+def convert_fleet_obstacles_batch(world, state, robot_world, fleet, N, T, E, dt, time_varying=False, order=True,
+                                  plan=False):
     """convert_world_obstacles_batch with the robots as obstacles of each other: robot b chooses from every shape of
     its world followed by every other robot of its world in ascending index, fleet [m] being robot m's shape (from
     fleet_shapes_batch).  robot_world [B] int32 or None (every robot in world 0).  Returns obs_A [B,N,Tc,E,2], obs_b [B,N,Tc,E], obs_kind [B,N], obs_count [B] (world
-    size plus the robots of the world minus one)."""
+    size plus the robots of the world minus one).  plan: the stage-t copy of a mate is its body along its plan,
+    fleet['plan_xy'][m, t] (from fleet_plan_shapes_batch), instead of its shape moved at constant velocity; the same
+    slots in the same order.  Needs time_varying."""
+    if plan and not time_varying:
+        raise ValueError('a fleet predicted along its plans needs time_varying=True')
     lib = _cabi.load()
     dev = state.device
     B, W = state.shape[0], world['start'].shape[0] - 1
@@ -283,15 +313,17 @@ def convert_fleet_obstacles_batch(world, state, robot_world, fleet, N, T, E, dt,
     b = torch.empty((B, N, Tc, E), dtype=torch.float32, device=dev)
     kind = torch.empty((B, N), dtype=torch.int32, device=dev)
     count = torch.empty(B, dtype=torch.int32, device=dev)
+    args = (B, W, N, T, E, dt, int(time_varying), int(order), _ptr(state), _ptr(world['start']), _ptr(robot_world),
+            _ptr(world['kind']), _ptr(world['nv']), _ptr(world['xy']), _ptr(world['radius']), _ptr(world['vel']),
+            _ptr(csr[0]), _ptr(csr[1]), _ptr(fleet['kind']), _ptr(fleet['nv']), _ptr(fleet['xy']), _ptr(fleet['radius']),
+            _ptr(fleet['vel']))
+    outs = (_ptr(A), _ptr(b), _ptr(kind), _ptr(count), _stream(dev))
     with torch.cuda.device(dev):
-        _cabi.check(lib.rda_convert_fleet_obstacles(B, W, N, T, E, dt, int(time_varying), int(order), _ptr(state),
-                                                    _ptr(world['start']), _ptr(robot_world), _ptr(world['kind']),
-                                                    _ptr(world['nv']), _ptr(world['xy']), _ptr(world['radius']),
-                                                    _ptr(world['vel']), _ptr(csr[0]), _ptr(csr[1]), _ptr(fleet['kind']),
-                                                    _ptr(fleet['nv']), _ptr(fleet['xy']), _ptr(fleet['radius']),
-                                                    _ptr(fleet['vel']), _ptr(A), _ptr(b), _ptr(kind), _ptr(count),
-                                                    _stream(dev)),
-                    'rda_convert_fleet_obstacles')
+        if plan:
+            _cabi.check(lib.rda_convert_fleet_plan_obstacles(*args, _ptr(fleet['plan_xy']), *outs),
+                        'rda_convert_fleet_plan_obstacles')
+        else:
+            _cabi.check(lib.rda_convert_fleet_obstacles(*args, *outs), 'rda_convert_fleet_obstacles')
     return A, b, kind, count
 
 
@@ -313,7 +345,9 @@ class BatchedMPC:
 
     control(avoid_fleet=True) makes the robots that share a map obstacles of each other: every other robot of the
     same map, its body at its current pose moving with the control it last applied, follows the map's shapes in the
-    list each robot chooses its N nearest obstacles from (convert_fleet_obstacles_batch).
+    list each robot chooses its N nearest obstacles from (convert_fleet_obstacles_batch).  With
+    fleet_prediction='plan' (and time_varying=True) each of them instead follows, stage by stage, the controls its own
+    last solve kept (cur_vel): the same obstacles in the same slots, turning, braking and stopping as planned.
 
     update_parameter(robots=mask, max_speed=..., ro2=...) gives robots their own limits, weights and tunables, so that
     robots of different classes (fast and slow, loaded and empty) step in one fleet and one solve.
@@ -437,17 +471,26 @@ class BatchedMPC:
         return self._empty
 
     def control(self, state, ref_speed=5.0, shapes=None, time_varying=False, world=None, robot_world=None,
-                avoid_fleet=False, clearance=False):
+                avoid_fleet=False, clearance=False, fleet_prediction='velocity'):
         """state [B,3] (CUDA tensor or array), ref_speed scalar or [B], shapes: dict from
         pack_shapes / shapes_to_device (None: free space).  Instead of shapes, world: dict from
         pack_worlds / shapes_to_device, obstacle maps shared by the robots, with robot_world [B] the map of
         each robot (may be omitted with a single map).  avoid_fleet: every robot also sees the other robots of its map
-        (without world: all robots, in an empty map) as moving obstacles; not with shapes.  Returns (u0 [B,2], info)
+        (without world: all robots, in an empty map) as moving obstacles; not with shapes.  fleet_prediction: how those
+        robots move over the horizon, 'velocity' (at the constant velocity of the control each just applied) or 'plan'
+        (along the controls its last solve kept, cur_vel; needs avoid_fleet and time_varying=True).  Returns (u0 [B,2], info)
         where info holds the solver's batched outputs plus 'arrive', 'nom_s', 'ref_s', 'cur_index', 'curve_index'.
         clearance: info also holds 'clearance' [B] and 'clearance_index' [B] of the plan just solved
         (RDA_solver.plan_clearance: the smallest signed distance between a robot's planned footprints and the obstacles
         it was given, negative inside one, and where it occurs).  No host sync."""
         dev, B, T = self.device, self.batch, self.T
+        if fleet_prediction not in ('velocity', 'plan'):
+            raise ValueError(f"fleet_prediction is 'velocity' or 'plan', not {fleet_prediction!r}")
+        plan = fleet_prediction == 'plan'
+        if plan and not avoid_fleet:
+            raise ValueError("fleet_prediction='plan' predicts the map-mates of avoid_fleet=True")
+        if plan and not time_varying:
+            raise ValueError("fleet_prediction='plan' needs time_varying=True: the prediction is a trajectory")
         if avoid_fleet:
             if shapes is not None:
                 raise ValueError('avoid_fleet takes its obstacles from world= (or an empty map), not from shapes')
@@ -492,9 +535,13 @@ class BatchedMPC:
             A, b, kind, count = self._no_obstacles()
             time_varying = False
         elif avoid_fleet:
-            fleet = fleet_shapes_batch(state, self.cur_vel, self.body, self.dynamics, self.per_robot)
+            if plan:
+                fleet = fleet_plan_shapes_batch(state, self.cur_vel, self.body, self.dynamics, self.dt, self.L,
+                                                self.per_robot)
+            else:
+                fleet = fleet_shapes_batch(state, self.cur_vel, self.body, self.dynamics, self.per_robot)
             A, b, kind, count = convert_fleet_obstacles_batch(world, state, robot_world, fleet, self.N, T, self.E,
-                                                              self.dt, time_varying, self.obstacle_order)
+                                                              self.dt, time_varying, self.obstacle_order, plan)
         elif world is not None:
             A, b, kind, count = convert_world_obstacles_batch(world, state, robot_world, self.N, T, self.E, self.dt,
                                                               time_varying, self.obstacle_order)
