@@ -6,6 +6,8 @@ import os
 
 import numpy as np
 
+from rda_planner_b200._cabi import DYNAMICS as _DYN
+
 from . import build_port
 
 
@@ -23,7 +25,6 @@ class _Tunables(C.Structure):
                 ('ro1', C.c_float), ('ro2', C.c_float), ('z_theta', C.c_float)]
 
 
-_DYN = {'acker': 0, 'diff': 1, 'omni': 2}
 _LIB = None
 
 
@@ -60,13 +61,11 @@ def host_threads():
     return {'effective': eff, 'affinity': aff, 'cgroup_quota': quota, 'os_cpu_count': os.cpu_count()}
 
 
-def solve_batch(car, T, N, E, nom_s, nom_u, ref_s, ref_speed, obs_A, obs_b, obs_kind, obs_count,
-                time_varying=False, iter_num=50, iter_threshold=0.0, dt=0.1, accelerated=True, threads=0,
-                **kw):
-    lib = _lib()
+def _config(car, T, N, E, B, dt, accelerated, **kw):
+    """The rda_config / rda_tunables pair of a solve of B instances: car's body, dynamics and limits, the weights and
+    tunables of kw (ws, wu, slack_gain, max_sd, min_sd, ro1, ro2, z_theta; RDA_solver's defaults for those left out)."""
     G = np.asarray(car.G, float); h = np.asarray(car.h, float).ravel()
     cfg = _Config()
-    B = int(np.asarray(nom_s).shape[0])
     cfg.batch, cfg.receding, cfg.max_obs_num, cfg.max_edge_num, cfg.robot_edges = B, T, N, E, G.shape[0]
     cfg.dynamics, cfg.accelerated, cfg.su_fp64 = _DYN[car.dynamics], int(accelerated), 1
     cfg.step_time, cfg.wheelbase = dt, float(car.wheelbase)
@@ -79,16 +78,37 @@ def solve_batch(car, T, N, E, nom_s, nom_u, ref_s, ref_speed, obs_A, obs_b, obs_
     cfg.robot_cone = 1 if getattr(car, 'cone_type', 'Rpositive') == 'norm2' else 0
     tun = _Tunables(kw.get('slack_gain', 8), kw.get('max_sd', 1.0), kw.get('min_sd', 0.1), kw.get('ro1', 200),
                     kw.get('ro2', 1), kw.get('z_theta', 0.5))
+    return cfg, tun
+
+
+def _inputs(nom_s, nom_u, ref_s, ref_speed, obs_A, obs_b, obs_kind, obs_count):
+    """The input arrays of port_solve_batch, contiguous, in its argument order."""
     f32 = lambda a: np.ascontiguousarray(a, np.float32)
     i32 = lambda a: np.ascontiguousarray(a, np.int32)
-    arrs = [f32(nom_s), f32(nom_u), f32(ref_s), f32(ref_speed), f32(obs_A), f32(obs_b), i32(obs_kind), i32(obs_count)]
-    u = np.zeros((B, 2, T), np.float32); s = np.zeros((B, 3, T + 1), np.float32)
-    rp = np.zeros(B, np.float32); rd = np.zeros(B, np.float32); it = np.zeros(B, np.int32)
-    fails = np.zeros((B, 4), np.int32)
-    p = lambda a: a.ctypes.data_as(C.c_void_p)
-    rc = lib.port_solve_batch(C.byref(cfg), C.byref(tun), C.c_int(B), *[p(a) for a in arrs], C.c_int(int(time_varying)),
-                              C.c_int(iter_num), C.c_float(iter_threshold), p(u), p(s), p(rp), p(rd), p(it), p(fails),
-                              C.c_int(threads))
+    return [f32(nom_s), f32(nom_u), f32(ref_s), f32(ref_speed), f32(obs_A), f32(obs_b), i32(obs_kind), i32(obs_count)]
+
+
+def _outputs(B, T):
+    """Zeroed output arrays of port_solve_batch, in its argument order, under the keys solve_batch returns."""
+    return {'u': np.zeros((B, 2, T), np.float32), 's': np.zeros((B, 3, T + 1), np.float32),
+            'resi_pri': np.zeros(B, np.float32), 'resi_dual': np.zeros(B, np.float32), 'iters': np.zeros(B, np.int32),
+            'cell_failures': np.zeros((B, 4), np.int32)}
+
+
+def _p(a):
+    return a.ctypes.data_as(C.c_void_p)
+
+
+def solve_batch(car, T, N, E, nom_s, nom_u, ref_s, ref_speed, obs_A, obs_b, obs_kind, obs_count,
+                time_varying=False, iter_num=50, iter_threshold=0.0, dt=0.1, accelerated=True, threads=0,
+                **kw):
+    lib = _lib()
+    B = int(np.asarray(nom_s).shape[0])
+    cfg, tun = _config(car, T, N, E, B, dt, accelerated, **kw)
+    arrs = _inputs(nom_s, nom_u, ref_s, ref_speed, obs_A, obs_b, obs_kind, obs_count)
+    out = _outputs(B, T)
+    rc = lib.port_solve_batch(C.byref(cfg), C.byref(tun), C.c_int(B), *map(_p, arrs), C.c_int(int(time_varying)),
+                              C.c_int(iter_num), C.c_float(iter_threshold), *map(_p, out.values()), C.c_int(threads))
     if rc != 0:
         raise RuntimeError(f'port_solve_batch: {rc}')
-    return {'u': u, 's': s, 'resi_pri': rp, 'resi_dual': rd, 'iters': it, 'cell_failures': fails}
+    return out

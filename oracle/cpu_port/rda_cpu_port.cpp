@@ -4,8 +4,11 @@
 //     arithmetic with the numpy oracle on a machine without a GPU;
 //   * port_solve_batch: the whole ADMM loop of rda_kernels.cu (k_begin / k_su / k_cells /
 //     k_finalize orchestration, float32 state, cold start) over a batch of instances with OpenMP
-//     over instances — the compiled multi-core CPU baseline bench.py reports ("port").
-// Never loaded by the product (rda_planner_b200/, RDA_planner/).
+//     over instances — the compiled multi-core CPU baseline bench.py reports ("port"), and the
+//     solver the CPU twins of tests/cpu_twin call per instance (declared in rda_cpu_port.h);
+//   * shim_pre_process, shim_convert_obstacles: the front end cores, one instance per call.
+// Built alone for bench.py (oracle/_build) and with tests/cpu_twin/*.cpp for the tests (tests/_build),
+// both by oracle/build_port.py.  Never loaded by the product (rda_planner_b200/, RDA_planner/).
 #include <vector>
 #include <cstring>
 #include <cmath>
@@ -16,28 +19,9 @@
 #include "../../rda_planner_b200/csrc/su_solver.cuh"
 #include "../../rda_planner_b200/csrc/cell_lean.cuh"
 #include "../../rda_planner_b200/csrc/cell_lean2.cuh"
-#ifdef RDA_CELL_STATS
-static void rda_coh_stat(int it, int lean_ok, int coh_ok);
-#endif
+#include "rda_cpu_port.h"
 
 using namespace rda;
-
-#ifdef RDA_SOC_STATS
-static long long g_soc[2];
-extern "C" void rda_soc_stat(int newton) {
-#pragma omp atomic
-  g_soc[0] += 1;
-#pragma omp atomic
-  g_soc[1] += newton;
-}
-static long long g_dr[4];
-extern "C" void rda_dr_stat(int what) {
-#pragma omp atomic
-  g_dr[what & 3] += 1;
-}
-extern "C" void port_dr_stats(long long* out) { for (int i = 0; i < 4; ++i) { out[i] = g_dr[i]; g_dr[i] = 0; } }
-extern "C" void port_soc_stats(long long* out, int reset) { out[0] = g_soc[0]; out[1] = g_soc[1]; if (reset) g_soc[0] = g_soc[1] = 0; }
-#endif
 
 template <typename Real>
 static int cell_impl(const float* G, const float* h, int R, int kind, int E, const float* A, const float* b,
@@ -214,9 +198,6 @@ int shim_su_report_f(const SuParams* P, const double* lins, const double* linu, 
 }
 
 
-static long long g_su_hist[64];
-extern "C" void port_su_hist(long long* out, int reset) { for (int i = 0; i < 64; ++i) { out[i] = g_su_hist[i]; if (reset) g_su_hist[i] = 0; } }
-
 // ------------------------------------------------------------------------------------------------
 // Whole hot path on the CPU (mirrors rda_kernels.cu; see the kernel comments for reference lines).
 // Layouts as in include/rda_b200.h.  Every instance starts cold (constructor state).
@@ -237,8 +218,7 @@ extern "C" int port_solve_batch(const rda_config* cfg, const rda_tunables* tun, 
   P.ab[0] = cfg->acce_bound[0]; P.ab[1] = cfg->acce_bound[1];
   P.ws = cfg->ws; P.wu = cfg->wu; P.slack_gain = tun->slack_gain; P.dmin = tun->min_sd; P.dmax = tun->max_sd;
   P.ro1 = tun->ro1; P.ro2 = tun->ro2; P.max_iter = 40;
-  P.mu0 = getenv("RDA_PORT_MU0") ? (float)atof(getenv("RDA_PORT_MU0")) : 1.0f;
-  P.prune = getenv("RDA_PORT_PRUNE") ? (float)atof(getenv("RDA_PORT_PRUNE")) : 0.5f;      // as the library default
+  P.mu0 = 1.0f; P.prune = 0.5f;      // as the library (rda_kernels.cu: mu0, the default su_prune)
   const float theta = cfg->accelerated ? tun->z_theta : 1.0f;
   if (nthreads > 0) omp_set_num_threads(nthreads);
   const size_t bytes = su_work_bytes<double>(T, N);
@@ -250,9 +230,6 @@ extern "C" int port_solve_batch(const rda_config* cfg, const rda_tunables* tun, 
     su_work_layout<double>(T, N, &W, base);
     std::vector<float> lam((size_t)N * E * T, 0.f), mu((size_t)N * R * T, 0.f), z(NT, 0.f), xi(2 * NT, 0.f),
         zeta(NT, 0.f), dis(T, 1.f), coef(5 * (size_t)NT, 0.f), pref(2 * T, 0.f);
-#ifdef RDA_CELL_STATS
-    std::vector<int> featv(NT > 0 ? NT : 1, 0);
-#endif
     const bool use_lean2 = getenv("RDA_PORT_LEAN2") && atoi(getenv("RDA_PORT_LEAN2")) != 0;
     std::vector<int> feat2(NT > 0 ? NT : 1, 0);
     std::vector<ObstacleGeom<4>> og2(N > 0 ? N : 1);
@@ -276,12 +253,6 @@ extern "C" int port_solve_batch(const rda_config* cfg, const rda_tunables* tun, 
       int nit = 0;
       const int st = su_solve<double, SeqCtx>(P, W, ctx, coef.data() + 3 * NT, coef.data() + 4 * NT, &nit);
       su_iters += nit;
-      if (W.restarts) {
-#pragma omp atomic
-        g_su_hist[0] += 1;      // slot 0 (never an iteration count): pruned solves that had to be repeated
-      }
-#pragma omp atomic
-      g_su_hist[nit < 63 ? nit : 63] += 1;
       if (st != 0) ++su_bad;
       if (st != 2) {
         for (int i = 0; i < 3 * (T + 1); ++i) { int r = i / (T + 1), t = i % (T + 1); cs[i] = (float)W.s[3 * t + r]; }
@@ -295,26 +266,6 @@ extern "C" int port_solve_batch(const rda_config* cfg, const rda_tunables* tun, 
             int tc = tv ? t + 1 : 0, Tc = tv ? T + 1 : 1;
             size_t ob = ((size_t)b * N + o) * Tc + tc;
             float ph = cs[2 * (T + 1) + t];
-#ifdef RDA_CELL_STATS
-            // emulation of the coherent first pass (cell_lean2.cuh): how often does the support-vertex pair of
-            // the previous ADMM iteration still certify the closest pair?  statistics only, results unused
-            if (E == 4 && R == 4 && !tv && obs_kind[(size_t)b * N + o] == RDA_OBS_POLYGON && xi[o * T + t] == 0.f && xi[NT + o * T + t] == 0.f) {
-              LeanOut<4, 4> l1, l2;
-              const bool ok1 = cell_lean<4, 4>(rb, RDA_OBS_POLYGON, E, obs_A + ob * E * 2, obs_b + ob * E, cs[t + 1], cs[(T + 1) + t + 1],
-                                               cosf(ph), sinf(ph), dis[t], zeta[o * T + t], 0.f, 0.f, theta, l1);
-              ObstacleGeom<4> og;
-              obstacle_geometry<4>(E, obs_A + ob * E * 2, obs_b + ob * E, og);
-              RobotAux ra;
-              robot_aux_from_geom(rb, &ra);
-              const int nf = cell_lean2<4, 4>(rb, ra, og, featv[o * T + t], cs[t + 1], cs[(T + 1) + t + 1], cosf(ph), sinf(ph), dis[t],
-                                              zeta[o * T + t], theta, l2);
-              rda_coh_stat(it, ok1 ? 1 : 0, nf >= 0 ? 1 : 0);
-              featv[o * T + t] = nf >= 0 ? nf : (ok1 ? l1.feat : 0);
-            } else {
-              rda_coh_stat(it, 0, 0);
-              featv[o * T + t] = 0;
-            }
-#endif
             CellOut<float> out;
             // emulation of the coherent pipeline (RDA_PORT_LEAN2=1): k_cells_coh -> listed cell_lean -> generic solver, under the
             // library's condition (rda_create / step_lammuz_part: E <= 4, R <= 4, static polygons; padded rows are zero)
@@ -410,40 +361,3 @@ extern "C" int shim_convert_obstacles(int M, int N, int T, int E, double dt, int
   }
   return count;
 }
-
-extern "C" void shim_motion_predict(int dynamics, double dt, double L, const double* s, double v0, double v1, double* out) {
-  rda::motion_predict(dynamics, dt, L, s, v0, v1, out);
-}
-
-// ---- statistics of the slow cell path (host analysis only; build with -DRDA_CELL_STATS) -------------
-#ifdef RDA_CELL_STATS
-namespace rda { long long g_cell_stats[8]; }     // which geometric situations reach the slow path (cell_solver.cuh)
-static long long g_stat_hist[3][512];
-extern "C" void rda_cell_stat(int what, int value) {
-  if (what < 0 || what > 2) return;
-  if (value < 0) value = 0;
-  if (value > 511) value = 511;
-#pragma omp atomic
-  g_stat_hist[what][value] += 1;
-}
-static long long g_case[1024];
-extern "C" void rda_case_stat(int line) {
-  if (line < 0 || line > 1023) return;
-#pragma omp atomic
-  g_case[line] += 1;
-}
-extern "C" void port_case_stats(long long* out) { memcpy(out, g_case, sizeof(g_case)); }
-static long long g_coh[64][3];
-static void rda_coh_stat(int it, int lean_ok, int coh_ok) {
-  if (it < 0 || it > 63) return;
-#pragma omp atomic
-  g_coh[it][0] += 1;
-#pragma omp atomic
-  g_coh[it][1] += lean_ok;
-#pragma omp atomic
-  g_coh[it][2] += coh_ok;
-}
-extern "C" void port_coh_stats(long long* out) { memcpy(out, g_coh, sizeof(g_coh)); }
-extern "C" void port_cell_stats(long long* out) { memcpy(out, g_stat_hist, sizeof(g_stat_hist)); }
-extern "C" void port_cell_situations(long long* out) { memcpy(out, rda::g_cell_stats, sizeof(rda::g_cell_stats)); }
-#endif

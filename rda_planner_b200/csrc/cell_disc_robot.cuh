@@ -14,11 +14,6 @@
 #pragma once
 #include "cell_solver.cuh"      // includes coop_ipm.cuh: coop_chol, tri_solve, the cooperative context interface
 
-#if defined(RDA_SOC_STATS) && !defined(__CUDA_ARCH__)
-extern "C" void rda_soc_stat(int newton);      // host statistics build only
-extern "C" void rda_dr_stat(int what);         // which cells reach the barrier programmes: 0 disjoint, 1 overlapping, +2 tilted
-#endif
-
 namespace rda {
 
 // min 1/2 x'Qx + c'x  s.t.  a_i'x <= b_i (i < m)  and  |(x[ia_k] + sa_k, x[ib_k] + sb_k)| <= (it_k >= 0 ? x[it_k] : 1), k < nc
@@ -163,9 +158,6 @@ RDA_HD bool soc_barrier(SocQP<NV, MC>& P, Ctx& ctx) {
     t = rmin(t * BARRIER_MU, BARRIER_TMAX);
   }
   if (lane == 0) P.newton = newton;
-#if defined(RDA_SOC_STATS) && !defined(__CUDA_ARCH__)
-  rda_soc_stat(newton);
-#endif
   return true;
 }
 
@@ -570,9 +562,6 @@ template <typename Real, typename Ctx>
 RDA_HD void cell_slow_dr(const RobotGeom& rb, CellWork<Real>& w, DiscSlowStore& S, Ctx& ctx) {
   const int lane = ctx.lane();
   const double rr = rb.rad, bcx = rb.cx, bcy = rb.cy;
-#if defined(RDA_SOC_STATS) && !defined(__CUDA_ARCH__)
-  rda_dr_stat((w.sep ? 0 : 1) + (w.xi_zero ? 0 : 2));
-#endif
   if (lane == 0) {
     const CellGeom<Real>& g = w.g;
     const double x0 = w.xi0, x1 = w.xi1, k0d = (double)w.k0, c_ = w.cphi, s_ = w.sphi;

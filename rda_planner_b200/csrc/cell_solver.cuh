@@ -16,13 +16,6 @@
 // Tie-break where the reference argmin is not unique: max margin, LP-vertex multipliers,
 // z = theta * max(stuff, 0).
 #pragma once
-// which closed form resolved a cell (host statistics build only)
-#if defined(RDA_CELL_STATS) && !defined(__CUDA_ARCH__)
-extern "C" void rda_case_stat(int line);
-#define RDA_CASE_STAT(line) rda_case_stat(line)
-#else
-#define RDA_CASE_STAT(line) ((void)0)
-#endif
 #include "rda_hd.h"
 
 namespace rda {
@@ -280,12 +273,12 @@ RDA_HD void cell_front(const RobotGeom& rb, int kind, int E, const float* A, con
       v0 = bdx / dist; v1 = bdy / dist;
       g0 = -(cphi * v0 + sphi * v1);
       g1 = -(-sphi * v0 + cphi * v1);
-      exact_zero_q = true; have = true; RDA_CASE_STAT(__LINE__); path = CELL_FAST_INACTIVE;
+      exact_zero_q = true; have = true; path = CELL_FAST_INACTIVE;
     }
   }
   if (!have && !sep && xi_zero && k0 <= 0) {
     // overlapping sets, no tilt: max margin is 0 at v = 0 (stuff = -k0 >= 0)
-    exact_zero_q = true; have = true; RDA_CASE_STAT(__LINE__); path = CELL_OVERLAP_FREE;
+    exact_zero_q = true; have = true; path = CELL_OVERLAP_FREE;
   }
   if (!have && sep) {
     const Real tolc = sizeof(Real) == 4 ? (Real)1e-5 : (Real)1e-11;
@@ -300,7 +293,7 @@ RDA_HD void cell_front(const RobotGeom& rb, int kind, int E, const float* A, con
         Real cgx = -rvx - xi0, cgy = -rvy - xi1;
         if (in_cone_rob<Real>(rb, j, cgx, cgy, tolc)) {
           v0 = vjx; v1 = vjy; g0 = cgx; g1 = cgy;
-          exact_zero_q = true; have = true; RDA_CASE_STAT(__LINE__); path = CELL_FAST_VERTEX;
+          exact_zero_q = true; have = true; path = CELL_FAST_VERTEX;
         }
       } else {
         Real tau = -Dj / ((Real)1 + (yx * yx + yy * yy) / ro2);
@@ -308,7 +301,7 @@ RDA_HD void cell_front(const RobotGeom& rb, int kind, int E, const float* A, con
         Real cgx = qx - rvx - xi0, cgy = qy - rvy - xi1;
         if (in_cone_rob<Real>(rb, j, cgx, cgy, tolc)) {
           v0 = vjx; v1 = vjy; g0 = cgx; g1 = cgy;
-          have = true; RDA_CASE_STAT(__LINE__); path = CELL_FAST_VERTEX;
+          have = true; path = CELL_FAST_VERTEX;
         }
       }
     }
@@ -431,7 +424,7 @@ RDA_HD void cell_front(const RobotGeom& rb, int kind, int E, const float* A, con
           const Real tang = abs_(cgx * fx + cgy * fy) * rsqrt_(fx * fx + fy * fy);
           if (cgx * (Real)rb.nx[j] + cgy * (Real)rb.ny[j] >= -tolc && tang <= tole) {
             v0 = vx_; v1 = vy_; g0 = cgx; g1 = cgy;
-            exact_zero_q = true; have = true; RDA_CASE_STAT(__LINE__); path = CELL_FAST_VERTEX;
+            exact_zero_q = true; have = true; path = CELL_FAST_VERTEX;
           }
         }
       } else if (Nv > 0) {
@@ -440,7 +433,7 @@ RDA_HD void cell_front(const RobotGeom& rb, int kind, int E, const float* A, con
         const Real tang = abs_(cgx * fx + cgy * fy) * rsqrt_(fx * fx + fy * fy);
         if (cgx * (Real)rb.nx[j] + cgy * (Real)rb.ny[j] >= -tolc && tang <= tole) {
           v0 = vx_; v1 = vy_; g0 = cgx; g1 = cgy;
-          have = true; RDA_CASE_STAT(__LINE__); path = CELL_FAST_VERTEX;
+          have = true; path = CELL_FAST_VERTEX;
         }
       }
     }
@@ -485,7 +478,7 @@ RDA_HD void cell_front(const RobotGeom& rb, int kind, int E, const float* A, con
         const Real tang = abs_(cgx * fx + cgy * fy) * rsqrt_(fx * fx + fy * fy);
         if (!(cgx * (Real)rb.nx[j] + cgy * (Real)rb.ny[j] >= -tolc && tang <= (Real)CELL_EE_TANG)) continue;
         v0 = nix; v1 = niy; g0 = cgx; g1 = cgy;
-        have = true; RDA_CASE_STAT(__LINE__); path = CELL_FAST_VERTEX;
+        have = true; path = CELL_FAST_VERTEX;
       }
     }
   }
@@ -510,7 +503,7 @@ RDA_HD void cell_front(const RobotGeom& rb, int kind, int E, const float* A, con
     }
     if (inside) {
       v0 = 0; v1 = 0; g0 = 0; g1 = 0;
-      exact_zero_q = false; have = true; RDA_CASE_STAT(__LINE__); path = CELL_OVERLAP_FREE;
+      exact_zero_q = false; have = true; path = CELL_OVERLAP_FREE;
     }
   }
   if (!have && !sep) {
@@ -548,7 +541,7 @@ RDA_HD void cell_front(const RobotGeom& rb, int kind, int E, const float* A, con
       const Real cgx = -tau * yx / ro2 - xi0, cgy = -tau * yy / ro2 - xi1;
       if (cgx * (Real)rb.nx[j] + cgy * (Real)rb.ny[j] < -tolc) continue;
       v0 = 0; v1 = 0; g0 = cgx; g1 = cgy;
-      have = true; RDA_CASE_STAT(__LINE__); path = CELL_OVERLAP_FREE;
+      have = true; path = CELL_OVERLAP_FREE;
     }
     // (iii) P(y) on obstacle edge i, y strictly inside the robot: g = 0, v = alpha n_i, 0 <= alpha <= 1
     if (kind != RDA_OBS_CIRCLE) {
@@ -578,7 +571,7 @@ RDA_HD void cell_front(const RobotGeom& rb, int kind, int E, const float* A, con
         if (!(alpha >= -tolc && alpha <= (Real)1 + tolc)) continue;
         const Real ac = rclamp(alpha, (Real)0, (Real)1);
         v0 = ac * g.nx[i]; v1 = ac * g.ny[i]; g0 = 0; g1 = 0;
-        have = true; RDA_CASE_STAT(__LINE__); path = CELL_OVERLAP_FREE;
+        have = true; path = CELL_OVERLAP_FREE;
       }
       // (iv) obstacle vertex i strictly inside the robot: y = R'V_i, g = 0, v = R(-tau y/ro2 - xi) must lie
       //      in the normal cone of the vertex with |v| <= 1
@@ -597,7 +590,7 @@ RDA_HD void cell_front(const RobotGeom& rb, int kind, int E, const float* A, con
         if (vx_ * epx + vy_ * epy < -tolc * sqrt_(epx * epx + epy * epy)) continue;
         if (vx_ * enx + vy_ * eny > tolc * sqrt_(enx * enx + eny * eny)) continue;
         v0 = vx_; v1 = vy_; g0 = 0; g1 = 0;
-        have = true; RDA_CASE_STAT(__LINE__); path = CELL_OVERLAP_FREE;
+        have = true; path = CELL_OVERLAP_FREE;
       }
       // (v) crossing of robot edge j and obstacle edge i: y fixed, g = gamma m_j, v = alpha n_i with
       //     gamma m_j + alpha R'n_i = -tau y/ro2 - xi  (2 x 2 linear system), gamma >= 0, 0 <= alpha <= 1
@@ -629,17 +622,11 @@ RDA_HD void cell_front(const RobotGeom& rb, int kind, int E, const float* A, con
           if (!(gam >= -tolc && alp >= -tolc && alp <= (Real)1 + tolc)) continue;
           const Real ac = rclamp(alp, (Real)0, (Real)1), gc = rmax(gam, (Real)0);
           v0 = ac * g.nx[i]; v1 = ac * g.ny[i]; g0 = gc * mjx; g1 = gc * mjy;
-          have = true; RDA_CASE_STAT(__LINE__); path = CELL_OVERLAP_FREE;
+          have = true; path = CELL_OVERLAP_FREE;
         }
       }
     }
   }
-#ifdef RDA_CELL_STATS
-  if (!have) {
-    extern long long g_cell_stats[8];
-    __sync_fetch_and_add(&g_cell_stats[(sep ? 0 : 2) + (xi_zero ? 0 : 1)], 1);
-  }
-#endif
   w.v0 = v0; w.v1 = v1; w.g0 = g0; w.g1 = g1;
   w.exact_zero_q = exact_zero_q; w.have = have; w.path = path;
 }

@@ -8,13 +8,6 @@
 // against the same cooperative context as su_solver.cuh (lane(), nlanes(), sync(), sum/min/max),
 // so that the g++ build (one lane) runs the identical arithmetic for the CPU tests.
 #pragma once
-// statistics hook of the host test build (oracle/cpu_port with -DRDA_CELL_STATS); a no-op everywhere else
-#if defined(RDA_CELL_STATS) && !defined(__CUDA_ARCH__)
-extern "C" void rda_cell_stat(int what, int value);
-#define RDA_STAT(what, value) rda_cell_stat(what, value)
-#else
-#define RDA_STAT(what, value) ((void)0)
-#endif
 #include "rda_hd.h"
 
 namespace rda {
@@ -141,10 +134,10 @@ RDA_HD bool coop_ipm(CoopQP<NV, MC>& P, Ctx& ctx) {
     }
     rdn = ctx.max(rdn); rpn = ctx.max(rpn);
     const double mu = ctx.sum(mus) / M;
-    if (!(rdn == rdn) || !(mu == mu)) { RDA_STAT(1, it); return false; }
+    if (!(rdn == rdn) || !(mu == mu)) return false;
     acceptable = rdn < 1e-6 * scale && rpn < 1e-6 * scale && mu < 1e-7;
-    if (rdn < 1e-9 * scale && rpn < 1e-9 * scale && mu < 1e-10) { RDA_STAT(0, it); return true; }
-    if (mu < 1e-14) { RDA_STAT(acceptable ? 0 : 1, it); return acceptable; }
+    if (rdn < 1e-9 * scale && rpn < 1e-9 * scale && mu < 1e-10) return true;
+    if (mu < 1e-14) return acceptable;
     ctx.sync();
     // ---- Newton matrix (lower triangle) and affine right-hand side ----
     const double wm = P.w[m];
@@ -175,7 +168,7 @@ RDA_HD bool coop_ipm(CoopQP<NV, MC>& P, Ctx& ctx) {
       P.ra[k] = v;
     }
     ctx.sync();
-    if (!coop_chol<NV, Ctx>(P.H, P.L, &P.flag, ctx)) { RDA_STAT(acceptable ? 0 : 1, it); return acceptable; }
+    if (!coop_chol<NV, Ctx>(P.H, P.L, &P.flag, ctx)) return acceptable;
     if (lane == 0) tri_solve<NV>(P.L, P.ra);
     ctx.sync();
     // ---- affine step: lengths and centring parameter ----
@@ -232,7 +225,6 @@ RDA_HD bool coop_ipm(CoopQP<NV, MC>& P, Ctx& ctx) {
     for (int i = lane; i < M; i += nl) { P.s[i] += alpha * P.ds[i]; P.l[i] += alpha * P.dl[i]; }
     ctx.sync();
   }
-  RDA_STAT(acceptable ? 0 : 1, 40);
   return acceptable;
 }
 
@@ -271,11 +263,9 @@ RDA_HD bool coop_barrier(CoopQP<NV, MC>& P, Ctx& ctx) {
   const int lane = ctx.lane(), nl = ctx.nlanes();
   const int m = P.m, tv = P.tv;
   double t = 1.0;
-  int newton = 0;
   for (int outer = 0; outer < 64; ++outer) {
     const bool last = t >= BARRIER_TMAX;
     for (int it = 0; it < 30; ++it) {
-      ++newton;
       // slack reciprocals
       for (int i = lane; i < m; i += nl) {
         double sl = P.b[i];
@@ -340,8 +330,6 @@ RDA_HD bool coop_barrier(CoopQP<NV, MC>& P, Ctx& ctx) {
     if (last) break;
     t = rmin(t * BARRIER_MU, BARRIER_TMAX);
   }
-  RDA_STAT(2, newton);
-  (void)newton;
   return true;
 }
 

@@ -4,7 +4,10 @@
 // the su-QP parameters (su_instance, k_admm_small) and inst_ro2 for the cells' ro2 (the listed cell passes).  Each
 // instance is then solved on its own: instances of a batch never interact.  Layouts as port_solve_batch; inst may be
 // NULL (the handle's values for every instance, port_solve_batch itself).
-#include "../../oracle/cpu_port/rda_cpu_port.cpp"
+#include "../../oracle/cpu_port/rda_cpu_port.h"
+#include "../../rda_planner_b200/csrc/su_solver.cuh"
+
+using namespace rda;
 
 extern "C" int twin_solve_batch_inst(const rda_config* cfg, const rda_tunables* tun, int B, const float* nom_s,
                                      const float* nom_u, const float* ref_s, const float* ref_speed, const float* obs_A,

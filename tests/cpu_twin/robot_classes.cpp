@@ -4,7 +4,11 @@
 // for the slot (an index outside [0, K) is the handle's own) and su_params_class for the su-QP's dynamics and wheelbase.
 // Each instance is then solved on its own: instances of a batch never interact.  Layouts as port_solve_batch;
 // robot_class may be NULL (the handle's own for every instance, port_solve_batch itself).
-#include "../../oracle/cpu_port/rda_cpu_port.cpp"
+#include <cstring>
+#include "../../oracle/cpu_port/rda_cpu_port.h"
+#include "../../rda_planner_b200/csrc/su_solver.cuh"
+
+using namespace rda;
 
 // limits: [K][4] max_speed[2], acce_bound[2] of each class (the per-instance table columns the classes set)
 extern "C" int twin_solve_batch_cls(const rda_config* cfg, const rda_tunables* tun, int B, const float* nom_s,

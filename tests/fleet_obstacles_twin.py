@@ -1,47 +1,14 @@
 """ctypes access to a g++ build of tests/cpu_twin/fleet_obstacles.cpp, the CPU twin of rda_fleet_shapes, and the
 selection of rda_convert_fleet_obstacles restated as the world twin (world_twin) over each robot's list: its world's
-shapes, then its map-mates — test infrastructure only.  Built on first use into tests/_build, or into a temporary
-directory when the tree is read-only."""
+shapes, then its map-mates — test infrastructure only."""
 import ctypes as C
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
+import shim
 import world_twin
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(HERE, 'cpu_twin', 'fleet_obstacles.cpp')
-CSRC = os.path.join(os.path.dirname(HERE), 'rda_planner_b200', 'csrc')
-INCLUDE = os.path.join(os.path.dirname(HERE), 'include', 'rda_b200.h')
-SO = os.path.join(HERE, '_build', 'libfleet_obstacles_twin.so')
-DYN = {'acker': 0, 'diff': 1, 'omni': 2}
 KEYS = ('kind', 'nv', 'xy', 'radius', 'vel')
-
-_lib = None
-
-
-def build():
-    deps = [SRC, INCLUDE] + [os.path.join(CSRC, f) for f in os.listdir(CSRC)]
-    if os.path.exists(SO) and all(os.path.getmtime(SO) >= os.path.getmtime(d) for d in deps):
-        return SO
-    so = SO
-    if not os.access(HERE, os.W_OK):
-        so = os.path.join(tempfile.mkdtemp(prefix='rda_fleet_obstacles_twin_'), os.path.basename(SO))
-    os.makedirs(os.path.dirname(so), exist_ok=True)
-    subprocess.check_call(['g++', '-O2', '-std=c++17', '-shared', '-fPIC', '-o', so, SRC])
-    return so
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        _lib = C.CDLL(build())
-        i, f, vp = C.c_int, C.c_float, C.c_void_p
-        _lib.shim_fleet_shapes.restype = None
-        _lib.shim_fleet_shapes.argtypes = [i, i, i, i, i, vp, f, vp, vp, vp, vp, vp, vp, vp]
-    return _lib
 
 
 def fleet_shapes(state, cur_vel, body, dynamics):
@@ -54,9 +21,12 @@ def fleet_shapes(state, cur_vel, body, dynamics):
            'radius': np.zeros(B, np.float32), 'vel': np.zeros((B, 2), np.float32)}
     bxy = np.ascontiguousarray(body['xy'], np.float32)
     p = lambda a: a.ctypes.data
-    lib().shim_fleet_shapes(B, T, DYN[dynamics], int(body['kind']), int(body['nv']), p(bxy), float(body['radius']),
-                            p(state), p(cur_vel), p(out['kind']), p(out['nv']), p(out['xy']), p(out['radius']),
-                            p(out['vel']))
+    i, f, vp = C.c_int, C.c_float, C.c_void_p
+    fn = shim.lib().shim_fleet_shapes
+    fn.restype = None
+    fn.argtypes = [i, i, i, i, i, vp, f, vp, vp, vp, vp, vp, vp, vp]
+    fn(B, T, shim.DYN[dynamics], int(body['kind']), int(body['nv']), p(bxy), float(body['radius']), p(state), p(cur_vel),
+       p(out['kind']), p(out['nv']), p(out['xy']), p(out['radius']), p(out['vel']))
     return out
 
 

@@ -1,48 +1,12 @@
 """ctypes access to a g++ build of tests/cpu_twin/fleet_plan.cpp, the CPU twin of rda_fleet_plan_shapes and of the
 selection of rda_convert_fleet_plan_obstacles over each robot's list (its world's shapes, then its map-mates along their
-plans) — test infrastructure only.  Built on first use into tests/_build, or into a temporary directory when the tree is
-read-only."""
+plans) — test infrastructure only."""
 import ctypes as C
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
 import fleet_obstacles_twin as ft
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(HERE, 'cpu_twin', 'fleet_plan.cpp')
-CSRC = os.path.join(os.path.dirname(HERE), 'rda_planner_b200', 'csrc')
-INCLUDE = os.path.join(os.path.dirname(HERE), 'include', 'rda_b200.h')
-SO = os.path.join(HERE, '_build', 'libfleet_plan_twin.so')
-DYN = {'acker': 0, 'diff': 1, 'omni': 2}
-
-_lib = None
-
-
-def build():
-    deps = [SRC, INCLUDE] + [os.path.join(CSRC, f) for f in os.listdir(CSRC)]
-    if os.path.exists(SO) and all(os.path.getmtime(SO) >= os.path.getmtime(d) for d in deps):
-        return SO
-    so = SO
-    if not os.access(HERE, os.W_OK):
-        so = os.path.join(tempfile.mkdtemp(prefix='rda_fleet_plan_twin_'), os.path.basename(SO))
-    os.makedirs(os.path.dirname(so), exist_ok=True)
-    subprocess.check_call(['g++', '-O2', '-std=c++17', '-shared', '-fPIC', '-o', so, SRC])
-    return so
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        _lib = C.CDLL(build())
-        i, f, d, vp = C.c_int, C.c_float, C.c_double, C.c_void_p
-        _lib.shim_fleet_plan_shapes.restype = None
-        _lib.shim_fleet_plan_shapes.argtypes = [i, i, i, d, d, i, i, vp, f] + [vp] * 12
-        _lib.shim_convert_plan_list.restype = i
-        _lib.shim_convert_plan_list.argtypes = [i, i, i, i, d, i] + [vp] * 11
-    return _lib
+import shim
 
 
 def fleet_plan_shapes(state, cur_vel, body, dynamics, dt, wheelbase, per_robot=None):
@@ -63,10 +27,13 @@ def fleet_plan_shapes(state, cur_vel, body, dynamics, dt, wheelbase, per_robot=N
               'radius': np.ascontiguousarray(per_robot['radius'], np.float32)}
     bxy = np.ascontiguousarray(body['xy'], np.float32)
     p = lambda a: None if a is None else a.ctypes.data
-    lib().shim_fleet_plan_shapes(B, T, DYN[dynamics], dt, wheelbase, int(body['kind']), int(body['nv']), p(bxy),
-                                 float(body['radius']), p(pr.get('dynamics')), p(pr.get('wheelbase')), p(pr.get('xy')),
-                                 p(pr.get('radius')), p(state), p(cur_vel), p(out['kind']), p(out['nv']), p(out['xy']),
-                                 p(out['radius']), p(out['vel']), p(out['plan_xy']))
+    i, f, d, vp = C.c_int, C.c_float, C.c_double, C.c_void_p
+    fn = shim.lib().shim_fleet_plan_shapes
+    fn.restype = None
+    fn.argtypes = [i, i, i, d, d, i, i, vp, f] + [vp] * 12
+    fn(B, T, shim.DYN[dynamics], dt, wheelbase, int(body['kind']), int(body['nv']), p(bxy), float(body['radius']),
+       p(pr.get('dynamics')), p(pr.get('wheelbase')), p(pr.get('xy')), p(pr.get('radius')), p(state), p(cur_vel),
+       p(out['kind']), p(out['nv']), p(out['xy']), p(out['radius']), p(out['vel']), p(out['plan_xy']))
     return out
 
 
@@ -95,6 +62,9 @@ def convert_fleet_plan_obstacles(world, fleet, robot_world, b, N, T, E, dt, orde
     k, nv = i32(lst['kind']), i32(lst['nv'])
     xy, rad, vel = f32(lst['xy']), f32(lst['radius']), f32(lst['vel'])
     p = lambda a: a.ctypes.data
-    cnt = lib().shim_convert_plan_list(count, N, T, E, dt, int(order), p(st), p(k), p(nv), p(xy), p(rad), p(vel),
-                                       p(planned), p(plan), p(A), p(bb), p(kind))
+    fn = shim.lib().shim_convert_plan_list
+    fn.restype = C.c_int
+    fn.argtypes = [C.c_int] * 4 + [C.c_double, C.c_int] + [C.c_void_p] * 11
+    cnt = fn(count, N, T, E, dt, int(order), p(st), p(k), p(nv), p(xy), p(rad), p(vel), p(planned), p(plan), p(A), p(bb),
+             p(kind))
     return A, bb, kind, cnt

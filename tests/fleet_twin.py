@@ -1,46 +1,10 @@
 """ctypes access to a g++ build of tests/cpu_twin/fleet_paths.cpp, the CPU twin of the per-robot path kernels
-(rda_pre_process_paths / rda_post_process_paths) — test infrastructure only.  Built on first use into tests/_build, or
-into a temporary directory when the tree is read-only."""
+(rda_pre_process_paths / rda_post_process_paths) — test infrastructure only."""
 import ctypes as C
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(HERE, 'cpu_twin', 'fleet_paths.cpp')
-CSRC = os.path.join(os.path.dirname(HERE), 'rda_planner_b200', 'csrc')
-INCLUDE = os.path.join(os.path.dirname(HERE), 'include', 'rda_b200.h')
-SO = os.path.join(HERE, '_build', 'libfleet_twin.so')
-DYN = {'acker': 0, 'diff': 1, 'omni': 2}
-
-_lib = None
-
-
-def build():
-    deps = [SRC, INCLUDE] + [os.path.join(CSRC, f) for f in os.listdir(CSRC)]
-    if os.path.exists(SO) and all(os.path.getmtime(SO) >= os.path.getmtime(d) for d in deps):
-        return SO
-    so = SO
-    if not os.access(HERE, os.W_OK):
-        so = os.path.join(tempfile.mkdtemp(prefix='rda_fleet_twin_'), os.path.basename(SO))
-    os.makedirs(os.path.dirname(so), exist_ok=True)
-    subprocess.check_call(['g++', '-O2', '-std=c++17', '-shared', '-fPIC', '-o', so, SRC])
-    return so
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        _lib = C.CDLL(build())
-        i, f, vp = C.c_int, C.c_float, C.c_void_p
-        _lib.shim_pre_process_paths.restype = None
-        _lib.shim_pre_process_paths.argtypes = [i, i, i, f, f, vp, vp, vp, vp, i, vp, vp, vp, vp, vp, vp, f, i, vp, vp,
-                                                vp, vp]
-        _lib.shim_post_process_paths.restype = None
-        _lib.shim_post_process_paths.argtypes = [i, i, i, vp, vp, vp, i, vp, vp, vp, vp, vp]
-    return _lib
+import shim
 
 
 def _f32(a):
@@ -65,9 +29,12 @@ def pre_process_paths(packed, dynamics, T, dt, L, state, cur_vel, ref_speed, rob
     near = np.zeros(B, np.int32)
     speed = np.zeros(B, np.float32)
     p = lambda a: a.ctypes.data
-    lib().shim_pre_process_paths(B, T, DYN[dynamics], dt, L, p(state), p(cur_vel), p(ref_speed), p(path), len(pc) - 1,
-                                 p(pc), p(cs), p(cg), p(rp), p(ci), p(si), threshold, ind_range, p(nom), p(ref),
-                                 p(near), p(speed))
+    i, f, vp = C.c_int, C.c_float, C.c_void_p
+    fn = shim.lib().shim_pre_process_paths
+    fn.restype = None
+    fn.argtypes = [i, i, i, f, f, vp, vp, vp, vp, i, vp, vp, vp, vp, vp, vp, f, i, vp, vp, vp, vp]
+    fn(B, T, shim.DYN[dynamics], dt, L, p(state), p(cur_vel), p(ref_speed), p(path), len(pc) - 1, p(pc), p(cs), p(cg),
+       p(rp), p(ci), p(si), threshold, ind_range, p(nom), p(ref), p(near), p(speed))
     return nom, ref, near, speed
 
 
@@ -79,6 +46,9 @@ def post_process_paths(packed, T, robot_path, goal_index_threshold, near_index, 
     cur_vel = np.zeros_like(u)
     arrive = np.zeros(B, np.int32)
     p = lambda a: a.ctypes.data
-    lib().shim_post_process_paths(B, T, len(pc) - 1, p(pc), p(cs), p(rp), goal_index_threshold, p(near), p(ci), p(u),
-                                  p(cur_vel), p(arrive))
+    i, vp = C.c_int, C.c_void_p
+    fn = shim.lib().shim_post_process_paths
+    fn.restype = None
+    fn.argtypes = [i, i, i, vp, vp, vp, i, vp, vp, vp, vp, vp]
+    fn(B, T, len(pc) - 1, p(pc), p(cs), p(rp), goal_index_threshold, p(near), p(ci), p(u), p(cur_vel), p(arrive))
     return near, ci, u, cur_vel, arrive

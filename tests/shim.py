@@ -1,6 +1,8 @@
-"""ctypes access to oracle/_build/librda_cpu_port.so (g++ build of the CUDA kernels' numerical
-cores, oracle/cpu_port) — test infrastructure only."""
+"""ctypes access to tests/_build/librda_twins.so: the g++ build of the CUDA kernels' numerical cores (oracle/cpu_port)
+linked with every CPU twin of tests/cpu_twin — test infrastructure only.  This module builds and loads the library; the
+*_twin modules wrap their own entry points of it.  A new twin is one tests/cpu_twin/*.cpp file."""
 import ctypes as C
+import glob
 import os
 import sys
 import numpy as np
@@ -8,6 +10,9 @@ import numpy as np
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 from oracle import build_port
+from rda_planner_b200._cabi import DYNAMICS as DYN
+
+SO = os.path.join(HERE, '_build', 'librda_twins.so')
 
 
 class SuParams(C.Structure):
@@ -19,7 +24,8 @@ class SuParams(C.Structure):
 
 
 def build(force=False):
-    return build_port.build(force)
+    srcs = [build_port.SRC] + sorted(glob.glob(os.path.join(HERE, 'cpu_twin', '*.cpp')))
+    return build_port.build_so(srcs, SO, force)
 
 
 _lib = None
@@ -42,9 +48,6 @@ def _f64(a):
 
 def _p(a):
     return a.ctypes.data_as(C.c_void_p)
-
-
-DYN = {'acker': 0, 'diff': 1, 'omni': 2}
 
 
 def cell(G, h, kind, A, b, p, phi, dbar, zeta, xi, ro2, theta=0.5, prec='d'):
