@@ -675,7 +675,7 @@ RDA_HD void cell_slow_dr(const RobotGeom& rb, CellWork<Real>& w, DiscSlowStore& 
 template <typename Real>
 RDA_HD void cell_back_dr(const RobotGeom& rb, const CellWork<Real>& w, Real zeta, Real theta, CellOut<Real>& out) {
   const CellGeom<Real>& g = w.g;
-  const int ne = g.ne, kind = g.kind;
+  const int kind = g.kind;
   const Real v0 = w.v0, v1 = w.v1, g0 = w.g0, g1 = w.g1, cphi = w.cphi, sphi = w.sphi;
   const Real xi0 = w.xi0, xi1 = w.xi1, k0 = w.k0;
   for (int i = 0; i < RDA_MAX_EDGE; ++i) out.lam[i] = 0;
@@ -692,12 +692,7 @@ RDA_HD void cell_back_dr(const RobotGeom& rb, const CellWork<Real>& w, Real zeta
   if (kind == RDA_OBS_CIRCLE) {
     out.lam[0] = v0; out.lam[1] = v1; out.lam[2] = -vn;
   } else if (vn > 0) {
-    const int a = (io + ne - 1) % ne, bb = io;
-    const Real det = g.nx[a] * g.ny[bb] - g.ny[a] * g.nx[bb];
-    const Real al = (v0 * g.ny[bb] - v1 * g.nx[bb]) / det;
-    const Real be = (g.nx[a] * v1 - g.ny[a] * v0) / det;
-    out.lam[a] = rmax(al, (Real)0) * g.inv_norm[a];
-    out.lam[bb] = rmax(be, (Real)0) * g.inv_norm[bb];
+    obs_vertex_lam<Real>(g, io, v0, v1, out.lam);
   }
   const Real gn = sqrt_(g0 * g0 + g1 * g1);
   out.mu[0] = g0; out.mu[1] = g1; out.mu[2] = -gn;                       // (g, -|g|): smallest mu'h in the cone

@@ -27,6 +27,17 @@ struct LeanOut {
   int feat;      // 0x40 | obstacle support vertex << 3 | robot support vertex of a separated polygon pair, else 0 (cell_lean2.cuh)
 };
 
+// LP-vertex coefficients (al, be) of a direction v at a vertex with rows of unit normals n_a, n_b: false when v lies clearly
+// outside the vertex's normal cone (the support went to the wrong end of a short edge) or al n_a + be n_b comes out longer
+// than v by more than rounding (rows nearly parallel).  The first passes then decline the cell, and the searched passes
+// resolve it (obs_vertex_lam, cell_solver.cuh).
+RDA_HD bool lp_vertex_ok(float nax, float nay, float nbx, float nby, float v0, float v1, float al, float be) {
+  if (rmin(al, be) < -1e-5f) return false;
+  al = rmax(al, 0.f); be = rmax(be, 0.f);
+  const float wx = al * nax + be * nbx, wy = al * nay + be * nby;
+  return wx * wx + wy * wy <= (v0 * v0 + v1 * v1) * (1.f + 1e-5f);
+}
+
 // returns true when the cell is resolved (outputs valid); false -> next pass
 template <int EC, int RC>
 RDA_HD bool cell_lean(const RobotGeom& rb, int kind, int E, const float* A, const float* b, float px, float py,
@@ -194,6 +205,7 @@ RDA_HD bool cell_lean(const RobotGeom& rb, int kind, int E, const float* A, cons
       const float det = anx * bny - any * bnx;
       const float al = (v0 * bny - v1 * bnx) / det;
       const float be = (anx * v1 - any * v0) / det;
+      if (!lp_vertex_ok(anx, any, bnx, bny, v0, v1, al, be)) return false;
       const float la = rmax(al, 0.f) * ain, lb = rmax(be, 0.f) * bin;
 #pragma unroll
       for (int i = 0; i < EC; ++i) lamv[i] = (i == ia) ? la : ((i == ib) ? lb : 0.f);

@@ -175,6 +175,7 @@ RDA_HD int cell_lean2(const RobotGeom& rb, const RobotAux& ra, const ObstacleGeo
   // LP-vertex multipliers at the two support vertices (precomputed 2x2 inverses)
   const int ia2 = (ib2 == 0) ? ne - 1 : ib2 - 1;
   const float al = v0 * og.pa0[ib2] + v1 * og.pa1[ib2], be = v0 * og.pb0[ib2] + v1 * og.pb1[ib2];
+  if (!lp_vertex_ok(og.nx[ia2], og.ny[ia2], og.nx[ib2], og.ny[ib2], v0, v1, al, be)) return -1;
   const float la = rmax(al, 0.f) * og.invn[ia2], lb = rmax(be, 0.f) * og.invn[ib2];
 #pragma unroll
   for (int i = 0; i < EC; ++i) out.lam[i] = (i == ia2) ? la : ((i == ib2) ? lb : 0.f);

@@ -96,6 +96,39 @@ RDA_HD Real support_rob(const RobotGeom& rb, Real gx, Real gy, int* arg) {
   return best;
 }
 
+// LP-vertex multipliers of the obstacle for the direction v = A'lam: v = al n_{a} + be n_{b} at the vertex joining rows a and b.
+// The two ends of a short edge have supports within |edge| of each other, and the vertex between two nearly parallel rows is
+// computed to a float32 error of eps |b| / det; so the support can go to the wrong end of a short edge.  v then lies outside
+// that vertex's normal cone: one coefficient is negative, and between nearly parallel rows the other is huge (|A'lam| = 26 on
+// a hull with a 1.2e-4 m edge).  A clearly negative coefficient therefore moves the vertex towards its row until v lies in
+// the cone.  At a correct support vertex nothing moves, so results there are unchanged.
+// Between rows delta apart the coefficients also carry a rounding error of eps / delta (the 2x2 determinant is delta), so
+// |al n_a + be n_b| can exceed |v| <= 1 by that much: cone_rescale (rda_hd.h) scales such a pair back to the length of v.
+template <typename Real>
+RDA_HD void obs_vertex_lam(const CellGeom<Real>& g, int io, Real v0, Real v1, Real* lam) {
+  const int ne = g.ne;
+  const Real tol = sizeof(Real) == 4 ? (Real)1e-5 : (Real)1e-11;
+  int a = (io + ne - 1) % ne, bb = io;
+  Real det = g.nx[a] * g.ny[bb] - g.ny[a] * g.nx[bb];
+  Real al = (v0 * g.ny[bb] - v1 * g.nx[bb]) / det;
+  Real be = (g.nx[a] * v1 - g.ny[a] * v0) / det;
+  if (rmin(al, be) < -tol) {
+    const bool back = be < al;            // v lies before row a: previous vertex; past row bb: next vertex
+    for (int s = 1; s < ne; ++s) {
+      if (back) { bb = a; a = (a + ne - 1) % ne; }
+      else { a = bb; bb = (bb + 1) % ne; }
+      det = g.nx[a] * g.ny[bb] - g.ny[a] * g.nx[bb];
+      al = (v0 * g.ny[bb] - v1 * g.nx[bb]) / det;
+      be = (g.nx[a] * v1 - g.ny[a] * v0) / det;
+      if ((back ? be : al) >= -tol) break;
+    }
+  }
+  al = rmax(al, (Real)0); be = rmax(be, (Real)0);
+  cone_rescale<Real>(g.nx[a], g.ny[a], g.nx[bb], g.ny[bb], v0, v1, al, be);
+  lam[a] = al * g.inv_norm[a];
+  lam[bb] = be * g.inv_norm[bb];
+}
+
 // g (body frame) inside the normal cone of body vertex j?
 template <typename Real>
 RDA_HD bool in_cone_rob(const RobotGeom& rb, int j, Real gx, Real gy, Real tol) {
@@ -777,7 +810,7 @@ RDA_HD void cell_slow(const RobotGeom& rb, CellWork<Real>& w, CellSlowStore& S, 
 template <typename Real>
 RDA_HD void cell_back(const RobotGeom& rb, const CellWork<Real>& w, Real zeta, Real theta, CellOut<Real>& out) {
   const CellGeom<Real>& g = w.g;
-  const int R = rb.R, ne = g.ne, kind = g.kind;
+  const int R = rb.R, kind = g.kind;
   const Real v0 = w.v0, v1 = w.v1, g0 = w.g0, g1 = w.g1, cphi = w.cphi, sphi = w.sphi;
   const Real xi0 = w.xi0, xi1 = w.xi1, k0 = w.k0;
   for (int i = 0; i < RDA_MAX_EDGE; ++i) out.lam[i] = 0;
@@ -796,12 +829,7 @@ RDA_HD void cell_back(const RobotGeom& rb, const CellWork<Real>& w, Real zeta, R
   if (kind == RDA_OBS_CIRCLE) {
     out.lam[0] = v0; out.lam[1] = v1; out.lam[2] = -vn;          // (v, -|v|), mpc.py:440-458
   } else if (vn > 0) {
-    int a = (io + ne - 1) % ne, bb = io;
-    Real det = g.nx[a] * g.ny[bb] - g.ny[a] * g.nx[bb];
-    Real al = (v0 * g.ny[bb] - v1 * g.nx[bb]) / det;
-    Real be = (g.nx[a] * v1 - g.ny[a] * v0) / det;
-    out.lam[a] = rmax(al, (Real)0) * g.inv_norm[a];
-    out.lam[bb] = rmax(be, (Real)0) * g.inv_norm[bb];
+    obs_vertex_lam<Real>(g, io, v0, v1, out.lam);
   }
   Real gn = sqrt_(g0 * g0 + g1 * g1);
   if (gn > 0) {

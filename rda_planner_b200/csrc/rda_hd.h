@@ -25,6 +25,15 @@ RDA_HD float sqrt_(float x) { return sqrtf(x); }
 RDA_HD double sqrt_(double x) { return sqrt(x); }
 RDA_HD float abs_(float x) { return fabsf(x); }
 RDA_HD double abs_(double x) { return fabs(x); }
+// LP-vertex coefficients (al, be) >= 0 of a direction v in the unit normals n_a, n_b of a vertex's two rows: scaled back to
+// |v| where al n_a + be n_b comes out longer than v by more than rounding (rows nearly parallel: the coefficients' rounding
+// error is eps / sin(angle between the rows)), so that |A'lam| <= |v| <= 1 holds as the reference's constraint requires
+template <typename T>
+RDA_HD void cone_rescale(T nax, T nay, T nbx, T nby, T v0, T v1, T& al, T& be) {
+  const T wx = al * nax + be * nbx, wy = al * nay + be * nby;
+  const T w2 = wx * wx + wy * wy, v2 = v0 * v0 + v1 * v1;
+  if (w2 > v2 * (T)(1 + 1e-5)) { const T f = sqrt_(v2 / w2); al *= f; be *= f; }
+}
 // reciprocal: on the device the hardware's double-precision reciprocal seed (MUFU.RCP64H, ~20 bits) refined by
 // two Newton steps — 5 dependent instructions, no float <-> double conversions (the float-seed variant of round
 // 1 spent 13 % of the su-QP kernel's stall samples on its two F2F conversions, profiles/ncu_r02_ksu_lines.md);
