@@ -16,6 +16,53 @@
 
 namespace rda {
 
+// sum and product rounded on their own, never fused with a neighbouring operation into an FMA: they keep an expression's
+// rounding where the compiler could otherwise contract differently (a factor of a constant +-1 folded away, an addend
+// held in a register instead of memory)
+RDA_HD float add_rn(float a, float b) {
+#if defined(__CUDA_ARCH__)
+  return __fadd_rn(a, b);
+#else
+  return a + b;
+#endif
+}
+RDA_HD double add_rn(double a, double b) {
+#if defined(__CUDA_ARCH__)
+  return __dadd_rn(a, b);
+#else
+  return a + b;
+#endif
+}
+// a * b + c fused on the device, where the compiler could otherwise leave it unfused (both arms of a branch merged into
+// one select); rounded twice on the host, as the host build computes it
+RDA_HD float fma_dev(float a, float b, float c) {
+#if defined(__CUDA_ARCH__)
+  return __fmaf_rn(a, b, c);
+#else
+  return a * b + c;
+#endif
+}
+RDA_HD double fma_dev(double a, double b, double c) {
+#if defined(__CUDA_ARCH__)
+  return __fma_rn(a, b, c);
+#else
+  return a * b + c;
+#endif
+}
+RDA_HD float mul_rn(float a, float b) {
+#if defined(__CUDA_ARCH__)
+  return __fmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+RDA_HD double mul_rn(double a, double b) {
+#if defined(__CUDA_ARCH__)
+  return __dmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
 template <typename T> RDA_HD T rmin(T a, T b) { return a < b ? a : b; }
 template <typename T> RDA_HD T rmax(T a, T b) { return a > b ? a : b; }
 template <typename T> RDA_HD T rclamp(T x, T lo, T hi) { return x < lo ? lo : (x > hi ? hi : x); }

@@ -187,9 +187,16 @@ __global__ void k_begin(DevPtrs d, const float* nom_s, const float* nom_u, const
 // W is laid out by the caller (hs / hnu and the workspace may live in shared or global memory).
 template <typename Real>
 __device__ __forceinline__ void su_instance(const DevPtrs& d, const SuParams& Ph, int b, SuWork<Real>& W, WarpCtx& ctx) {
-  SuParams P = Ph;
-  if (d.inst) su_params_row(P, d.inst + (size_t)b * RDA_INST_PARAMS);     // the instance's own row
-  if (d.cls) su_params_class(P, d.cls_kin[class_slot(d.cls, d.ncls, b)]);  // its class's dynamics and wheelbase
+  // The instance's parameters in the workspace: a local copy would be held in registers across the whole solve (and
+  // spill) or live in a stack frame read by local-memory loads.
+  if (ctx.lane() == 0) {
+    SuParams Pl = Ph;
+    if (d.inst) su_params_row(Pl, d.inst + (size_t)b * RDA_INST_PARAMS);     // the instance's own row
+    if (d.cls) su_params_class(Pl, d.cls_kin[class_slot(d.cls, d.ncls, b)]);  // its class's dynamics and wheelbase
+    *W.par = Pl;
+  }
+  ctx.sync();
+  const SuParams& P = *W.par;
   const int T = P.T, N = P.N, NT = N * T;
   const int lane = ctx.lane();
   const float* cs = d.cur_s + (size_t)b * 3 * (T + 1);   // [3][T+1]

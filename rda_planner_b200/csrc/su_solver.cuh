@@ -91,6 +91,8 @@ struct SuWork {
                               // consumed by the factorising backward sweep of the predictor, the affine
                               // step is produced by the forward sweep that follows it and is dead before
                               // the next predictor assembles (Wm, wb) again.
+  Real *lim;                  // 6   limits of the box and rate rows (su_limits)
+  SuParams *par;              // the instance's parameters: the kernels keep their copy here, in fast memory
   Real vref;
   int restarts;               // out: 1 when the pruned solve failed its verification and was repeated with all hinges
 };
@@ -137,7 +139,7 @@ RDA_HD size_t su_work_layout(int T, int N, SuWork<Real>* w, char* base, bool hin
   RDA_TAKE_S(Ed, 3 * T, Real) RDA_TAKE_S(g5q, T, Real)
   RDA_TAKE_S(gw, 8 * T + 5, Real)                                     // gw | (dz, dv)
   if (w) { w->dz = w->gw; w->dv = w->gw + 5 * (T + 1); }
-  RDA_TAKE_S(K, 10 * T, Real) RDA_TAKE_S(Lc, 3 * T, Real) RDA_TAKE_S(kf, 2 * T, Real)
+  RDA_TAKE_S(lim, 6, Real) RDA_TAKE_S(par, 1, SuParams) RDA_TAKE_S(K, 10 * T, Real) RDA_TAKE_S(Lc, 3 * T, Real) RDA_TAKE_S(kf, 2 * T, Real)
   if (w) { w->Cj = w->K; w->linu = (float*)w->dv; }
 #undef RDA_TAKE_S
 #undef RDA_TAKE_G
@@ -181,46 +183,43 @@ RDA_HD void su_linearise(const SuParams& P, const Real* st, const Real* ut, Real
   }
 }
 
-// One inequality row of stage t.  c in 0..9: (u0 hi, u0 lo, u1 hi, u1 lo, d hi, d lo,
-// rate0 hi, rate0 lo, rate1 hi, rate1 lo).  value g >= 0, gradient = sgn on component `comp`
-// (3: u0, 4: u1, 5: d) and -sgn on the previous control for rate rows.
-template <typename Real>
-struct Row { Real g; Real sgn; int comp; bool rate; bool live; };
+// The ten box and rate rows of stage t come as five (hi, lo) pairs, each of one direction x:
+//   u0: x = u_t[0],  g = umax0 - x | x + umax0        u1: x = u_t[1], likewise with umax1
+//   d:  x = d_t,     g = dmax - x  | x - max(dmin, 0)  (dead when N = 0)
+//   rate_k: x = u_t[k] - u_{t-1}[k], g = ab_k - x | ab_k + x   (dead at t = 0)
+// Row values g >= 0; the hi row's gradient is -1 along x, the lo row's +1.  Rows are numbered c = 0..9 in the order
+// u0 hi, u0 lo, u1 hi, u1 lo, d hi, d lo, rate0 hi, rate0 lo, rate1 hi, rate1 lo (the slot of (bs, bnu) at 10 t + c), and
+// every pass takes them in that order.  Everything is named scalars: no array indexed at run time, so nothing of the
+// passes goes to the stack.
 
+// the rows' limits (umax0, umax1, dmax, max(dmin, 0), ab0, ab1), converted once per solve into the workspace.  Kept in
+// fast memory rather than in registers: six more values live across the Riccati sweeps make k_su<double> spill.
 template <typename Real>
-RDA_HD Row<Real> su_row(const SuParams& P, const SuWork<Real>& W, int t, int c) {
-  Row<Real> r;
-  r.rate = c >= 6;
-  r.live = true;
-  const bool hi = (c & 1) == 0;
-  r.sgn = hi ? (Real)-1 : (Real)1;
-  if (c < 4) {
-    int k = c >> 1;
-    r.comp = 3 + k;
-    Real uv = W.u[2 * t + k], m = P.umax[k];
-    r.g = hi ? m - uv : uv + m;
-  } else if (c < 6) {
-    r.comp = 5;
-    Real dv = W.d[t];
-    Real lo = P.dmin > 0 ? P.dmin : 0;
-    r.g = hi ? (Real)P.dmax - dv : dv - lo;
-    r.live = P.N > 0;
-  } else {
-    int k = (c - 6) >> 1;
-    r.comp = 3 + k;
-    r.live = t >= 1;
-    Real du = r.live ? W.u[2 * t + k] - W.u[2 * (t - 1) + k] : (Real)0;
-    r.g = hi ? (Real)P.ab[k] - du : (Real)P.ab[k] + du;
-  }
-  return r;
+RDA_HD void su_limits(const SuParams& P, SuWork<Real>& W) {
+  const float dlo = P.dmin > 0 ? P.dmin : 0;
+  W.lim[0] = P.umax[0]; W.lim[1] = P.umax[1]; W.lim[2] = P.dmax; W.lim[3] = dlo; W.lim[4] = P.ab[0]; W.lim[5] = P.ab[1];
 }
 
-// directional derivative of row (t, c) along the Newton step held in (dz, dv)
+// row values of stage t at the iterate (u, d)
 template <typename Real>
-RDA_HD Real su_row_dir(const Row<Real>& r, const Real* dz_t, const Real* dv_t) {
-  Real x = dv_t[r.comp - 3];
-  if (r.rate) x -= dz_t[3 + (r.comp - 3)];
-  return r.sgn * x;
+struct SuRows { Real u0h, u0l, u1h, u1l, dh, dl, r0h, r0l, r1h, r1l; };
+
+template <typename Real>
+RDA_HD SuRows<Real> su_rows(const SuWork<Real>& W, int t) {
+  const Real u0 = W.u[2 * t], u1 = W.u[2 * t + 1], d = W.d[t];
+  const Real du0 = t >= 1 ? u0 - W.u[2 * t - 2] : (Real)0, du1 = t >= 1 ? u1 - W.u[2 * t - 1] : (Real)0;
+  const Real umax0 = W.lim[0], umax1 = W.lim[1], dmax = W.lim[2], dlo = W.lim[3], ab0 = W.lim[4], ab1 = W.lim[5];
+  return {umax0 - u0, u0 + umax0, umax1 - u1, u1 + umax1, dmax - d, d - dlo,
+          ab0 - du0, ab0 + du0, ab1 - du1, ab1 + du1};
+}
+
+// the pairs' directions along the Newton step (dz_t, dv_t) of stage t
+template <typename Real>
+struct SuDirs { Real u0, u1, d, r0, r1; };
+
+template <typename Real>
+RDA_HD SuDirs<Real> su_dirs(const Real* dz_t, const Real* dv_t) {
+  return {dv_t[0], dv_t[1], dv_t[2], dv_t[0] - dz_t[3], dv_t[1] - dz_t[4]};
 }
 
 template <typename Real, typename Ctx>
@@ -364,6 +363,7 @@ RDA_HD int su_solve(const SuParams& P, SuWork<Real>& W, Ctx& ctx, const float* g
   const Real ro1 = P.ro1, ro2 = P.ro2;
   const Real iro1 = (Real)1 / ro1;
   const bool acc = P.accelerated != 0;
+  if (lane == 0) su_limits<Real>(P, W);        // read by every lane after the sync that ends the linearisation
   // ---- linearisation and aggregated rotation terms (lane-parallel over stages) ----
   for (int t = lane; t < T; t += nl) {
     const Real st[3] = {(Real)W.lins[3 * t], (Real)W.lins[3 * t + 1], (Real)W.lins[3 * t + 2]};
@@ -417,12 +417,18 @@ RDA_HD int su_solve(const SuParams& P, SuWork<Real>& W, Ctx& ctx, const float* g
   const Real mu0 = P.mu0 > 0 ? (Real)P.mu0 : (Real)1;
   int nrows = 0;
   for (int t = lane; t < T; t += nl) {
-    _Pragma("unroll 1") for (int c = 0; c < 10; ++c) {
-      Row<Real> r = su_row<Real>(P, W, t, c);
-      Real sv = r.live ? rmax(r.g, (Real)1e-2) : (Real)1;
-      W.bs[10 * t + c] = sv;
-      W.bnu[10 * t + c] = r.live ? mu0 / sv : (Real)0;
-      if (r.live) ++nrows;
+    {
+      const SuRows<Real> R = su_rows<Real>(W, t);
+      auto row = [&](int c, Real g, bool live) {
+        Real sv = live ? rmax(g, (Real)1e-2) : (Real)1;
+        W.bs[10 * t + c] = sv;
+        W.bnu[10 * t + c] = live ? mu0 / sv : (Real)0;
+        if (live) ++nrows;
+      };
+      const bool dlive = N > 0, rlive = t >= 1;
+      row(0, R.u0h, true); row(1, R.u0l, true); row(2, R.u1h, true); row(3, R.u1l, true);
+      row(4, R.dh, dlive); row(5, R.dl, dlive);
+      row(6, R.r0h, rlive); row(7, R.r0l, rlive); row(8, R.r1h, rlive); row(9, R.r1l, rlive);
     }
     if (acc) {
       Real dx = W.s[3 * t + 3] - W.pref[2 * t], dy = W.s[3 * t + 4] - W.pref[2 * t + 1];
@@ -481,43 +487,62 @@ RDA_HD int su_solve(const SuParams& P, SuWork<Real>& W, Ctx& ctx, const float* g
         Real* gw = W.gw + 8 * t;
         const Real* sn = W.s + 3 * t + 3;
         const Real tw = 2 * (Real)P.ws;
-        gw[0] = tw * (sn[0] - W.ref[3 * t + 3]);
-        gw[1] = tw * (sn[1] - W.ref[3 * t + 4]);
-        gw[2] = (P.dynamics == RDA_DYN_OMNI ? (Real)0 : tw * (sn[2] - W.ref[3 * t + 5]))
-                + ro2 * (W.Skk[t] * (sn[2] - W.lins[3 * t + 2]) + W.Sgk[t]);
-        gw[3] = 2 * (Real)P.wu * (W.u[2 * t] - W.vref) + reg * W.u[2 * t];
-        gw[4] = reg * W.u[2 * t + 1];
-        gw[5] = N > 0 ? -(Real)P.slack_gain + reg * W.d[t] : (Real)0;
-        gw[6] = 0; gw[7] = 0;
-        Real wb[5] = {0, 0, 0, 0, 0};
-        _Pragma("unroll 1") for (int c = 0; c < 10; ++c) {
-          Row<Real> r = su_row<Real>(P, W, t, c);
-          if (!r.live) continue;
-          Real sv = W.bs[10 * t + c], nu = W.bnu[10 * t + c];
-          Real res = r.g - sv;
-          const Real isv = rcp_(sv);
-          Real om = nu * isv;
-          Real term;
-          if (phase == 0) {
-            term = -om * res;
-            acc_mu += sv * nu;
-            acc_r = rmax(acc_r, abs_(res));
-          } else {
-            Real dir = su_row_dir<Real>(r, W.dza + 5 * t, W.dva + 3 * t);
-            Real dsa = dir + res;
-            Real dna = -nu - om * dsa;
-            term = (sigma_mu - dsa * dna) * isv - om * res;
+        // gradient in registers: gw[0..4], gw[5] (d_t) and the rate terms gw[6..7] on the previous control.  Products that
+        // start a sum are rounded on their own (mul_rn), as when the sum started from a value in memory.
+        Real g0 = mul_rn(tw, sn[0] - (Real)W.ref[3 * t + 3]);
+        Real g1 = mul_rn(tw, sn[1] - (Real)W.ref[3 * t + 4]);
+        const Real g2 = (P.dynamics == RDA_DYN_OMNI ? (Real)0 : tw * (sn[2] - W.ref[3 * t + 5]))
+                        + ro2 * (W.Skk[t] * (sn[2] - W.lins[3 * t + 2]) + W.Sgk[t]);
+        Real g3 = 2 * (Real)P.wu * (W.u[2 * t] - W.vref) + reg * W.u[2 * t];
+        Real g4 = mul_rn(reg, W.u[2 * t + 1]);
+        Real g5 = N > 0 ? -(Real)P.slack_gain + reg * W.d[t] : (Real)0;
+        Real g6 = 0, g7 = 0;
+        Real wb2 = 0;                                // barrier weight of d_t (the Schur complement below)
+        {
+          Real wb0 = 0, wb1 = 0, wb3 = 0, wb4 = 0;
+          const SuRows<Real> R = su_rows<Real>(W, t);
+          SuDirs<Real> xa = {0, 0, 0, 0, 0};     // corrector: the pairs' directions along the affine step
+          if (phase == 1) xa = su_dirs<Real>(W.dza + 5 * t, W.dva + 3 * t);
+          // row c: g -= grad * term on the pair's component gc; adds om to the pair's barrier weight wbk and returns
+          // sgn * term (a rate row's term on the previous control).  The gradient sums are add_rn: with the sign a
+          // constant, the compiler would otherwise fuse them into the FMAs of term and round differently.
+          auto row = [&](int c, Real g, Real sgn, Real x, Real& gc, Real& wbk) {
+            const Real sv = W.bs[10 * t + c], nu = W.bnu[10 * t + c];
+            const Real res = g - sv;
+            const Real isv = rcp_(sv);
+            const Real om = nu * isv;
+            Real term;
+            if (phase == 0) {
+              term = -om * res;
+              acc_mu += sv * nu;
+              acc_r = rmax(acc_r, abs_(res));
+            } else {
+              const Real dir = sgn * x;
+              const Real dsa = dir + res;
+              const Real dna = -nu - om * dsa;
+              term = (sigma_mu - dsa * dna) * isv - om * res;
+            }
+            const Real gt = sgn * term;
+            gc = add_rn(gc, -gt);
+            if (phase == 0) wbk += om;
+            return gt;
+          };
+          row(0, R.u0h, -1, xa.u0, g3, wb0); row(1, R.u0l, 1, xa.u0, g3, wb0);
+          row(2, R.u1h, -1, xa.u1, g4, wb1); row(3, R.u1l, 1, xa.u1, g4, wb1);
+          if (N > 0) { row(4, R.dh, -1, xa.d, g5, wb2); row(5, R.dl, 1, xa.d, g5, wb2); }
+          if (t >= 1) {
+            g6 = add_rn(g6, row(6, R.r0h, -1, xa.r0, g3, wb3)); g6 = add_rn(g6, row(7, R.r0l, 1, xa.r0, g3, wb3));
+            g7 = add_rn(g7, row(8, R.r1h, -1, xa.r1, g4, wb4)); g7 = add_rn(g7, row(9, R.r1l, 1, xa.r1, g4, wb4));
           }
-          // g -= grad * term
-          gw[r.comp] -= r.sgn * term;
-          if (r.rate) gw[r.comp + 3] += r.sgn * term;
-          if (phase == 0) wb[(r.rate ? 3 : 0) + (r.comp - 3)] += om;
+          if (phase == 0) {
+            Real* wb = W.wb + 5 * t;
+            wb[0] = wb0; wb[1] = wb1; wb[2] = wb2; wb[3] = wb3; wb[4] = wb4;
+          }
+          gw[2] = g2; gw[3] = g3; gw[4] = g4; gw[6] = g6; gw[7] = g7;
         }
-        if (phase == 0) for (int k = 0; k < 5; ++k) W.wb[5 * t + k] = wb[k];
         Real m0 = 0, m1 = 0, m2 = 0, m3 = 0, m4 = 0, m5 = 0;
         Real dx = sn[0] - W.pref[2 * t], dy = sn[1] - W.pref[2 * t + 1];
         Real dd = W.d[t];
-        Real g0 = gw[0], g1 = gw[1], g5 = gw[5];     // accumulated in registers: no store inside the hinge loop
         // hinges in chunks of RDA_SU_CH: all (global-memory) loads of a chunk are issued before its arithmetic
         const Real adx = phase == 1 ? W.dza[5 * t + 5] : (Real)0, ady = phase == 1 ? W.dza[5 * t + 6] : (Real)0;
         const Real add = phase == 1 ? W.dva[3 * t + 2] : (Real)0;
@@ -566,7 +591,7 @@ RDA_HD int su_solve(const SuParams& P, SuWork<Real>& W, Ctx& ctx, const float* g
         }
         // eliminate d_t (it enters stage t only): Schur complement on Q_dd = reg + barrier weights + sum om
         if (phase == 0) {
-          const Real iq = N > 0 ? rcp_(reg + wb[2] + m5) : (Real)1;
+          const Real iq = N > 0 ? rcp_(reg + wb2 + m5) : (Real)1;
           const Real e0 = m2 * iq, e1 = m4 * iq;
           Real* M = W.Wm + 3 * t;
           M[0] = m0 - m2 * e0; M[1] = m1 - m2 * e1; M[2] = m3 - m4 * e1;
@@ -593,24 +618,36 @@ RDA_HD int su_solve(const SuParams& P, SuWork<Real>& W, Ctx& ctx, const float* g
       const Real* dv = phase == 0 ? W.dva : W.dv;
       Real rmaxr = 0, s0 = 0, s1 = 0, s2 = 0;   // rmaxr = max over rows of (-delta / value): 1 / max step
       for (int t = lane; t < T; t += nl) {
-        _Pragma("unroll 1") for (int c = 0; c < 10; ++c) {
-          Row<Real> r = su_row<Real>(P, W, t, c);
-          if (!r.live) continue;
-          Real sv = W.bs[10 * t + c], nu = W.bnu[10 * t + c];
-          Real res = r.g - sv;
-          Real dir = su_row_dir<Real>(r, dz + 5 * t, dv + 3 * t);
-          Real ds = dir + res, dn;
-          const Real ip = rcp_(sv * nu);
-          const Real isv = nu * ip, inu = sv * ip, om = nu * isv;
-          if (phase == 0) dn = -nu - om * ds;
-          else {
-            Real dira = su_row_dir<Real>(r, W.dza + 5 * t, W.dva + 3 * t);
-            Real dsa = dira + res;
-            Real dna = -nu - om * dsa;
-            dn = (sigma_mu - dsa * dna) * isv - nu - om * ds;
+        {
+          const SuRows<Real> R = su_rows<Real>(W, t);
+          const SuDirs<Real> x = su_dirs<Real>(dz + 5 * t, dv + 3 * t);
+          SuDirs<Real> xa = {0, 0, 0, 0, 0};
+          if (phase == 1) xa = su_dirs<Real>(W.dza + 5 * t, W.dva + 3 * t);
+          auto row = [&](int c, Real g, Real sgn, Real xs, Real xas) {
+            const Real sv = W.bs[10 * t + c], nu = W.bnu[10 * t + c];
+            const Real res = g - sv;
+            const Real dir = sgn * xs;
+            const Real ds = dir + res;
+            Real dn;
+            const Real ip = rcp_(sv * nu);
+            const Real isv = nu * ip, inu = sv * ip, om = nu * isv;
+            if (phase == 0) dn = -nu - om * ds;
+            else {
+              const Real dira = sgn * xas;
+              const Real dsa = dira + res;
+              const Real dna = -nu - om * dsa;
+              dn = fma_dev(sigma_mu - dsa * dna, isv, -nu) - om * ds;
+            }
+            rmaxr = rmax(rmaxr, rmax(-ds * isv, -dn * inu));
+            s0 += sv * nu; s1 += sv * dn + nu * ds; s2 += ds * dn;
+          };
+          row(0, R.u0h, -1, x.u0, xa.u0); row(1, R.u0l, 1, x.u0, xa.u0);
+          row(2, R.u1h, -1, x.u1, xa.u1); row(3, R.u1l, 1, x.u1, xa.u1);
+          if (N > 0) { row(4, R.dh, -1, x.d, xa.d); row(5, R.dl, 1, x.d, xa.d); }
+          if (t >= 1) {
+            row(6, R.r0h, -1, x.r0, xa.r0); row(7, R.r0l, 1, x.r0, xa.r0);
+            row(8, R.r1h, -1, x.r1, xa.r1); row(9, R.r1l, 1, x.r1, xa.r1);
           }
-          rmaxr = rmax(rmaxr, rmax(-ds * isv, -dn * inu));
-          s0 += sv * nu; s1 += sv * dn + nu * ds; s2 += ds * dn;
         }
         if (acc) {
           const Real dx = W.s[3 * t + 3] - W.pref[2 * t], dy = W.s[3 * t + 4] - W.pref[2 * t + 1], dd = W.d[t];
@@ -666,23 +703,29 @@ RDA_HD int su_solve(const SuParams& P, SuWork<Real>& W, Ctx& ctx, const float* g
 #endif
         // ---- update (needs the corrector quantities once more) ----
         for (int t = lane; t < T; t += nl) {
-          // rows first: they read the OLD iterate through su_row
-          Real gsave[10];
-          _Pragma("unroll 1") for (int c = 0; c < 10; ++c) { Row<Real> r = su_row<Real>(P, W, t, c); gsave[c] = r.g; }
-          _Pragma("unroll 1") for (int c = 0; c < 10; ++c) {
-            Row<Real> r = su_row<Real>(P, W, t, c);
-            if (!r.live) continue;
-            Real sv = W.bs[10 * t + c], nu = W.bnu[10 * t + c];
-            Real res = gsave[c] - sv;
-            Real dir = su_row_dir<Real>(r, W.dz + 5 * t, W.dv + 3 * t);
-            Real ds = dir + res;
-            Real dira = su_row_dir<Real>(r, W.dza + 5 * t, W.dva + 3 * t);
-            Real dsa = dira + res;
-            const Real isv = rcp_(sv), om = nu * isv;
-            Real dna = -nu - om * dsa;
-            Real dn = (sigma_mu - dsa * dna) * isv - nu - om * ds;
-            W.bs[10 * t + c] = sv + a * ds;
-            W.bnu[10 * t + c] = nu + a * dn;
+          {
+            const SuRows<Real> R = su_rows<Real>(W, t);      // at the old iterate (updated after the sync below)
+            const SuDirs<Real> x = su_dirs<Real>(W.dz + 5 * t, W.dv + 3 * t), xa = su_dirs<Real>(W.dza + 5 * t, W.dva + 3 * t);
+            auto row = [&](int c, Real g, Real sgn, Real xs, Real xas) {
+              const Real sv = W.bs[10 * t + c], nu = W.bnu[10 * t + c];
+              const Real res = g - sv;
+              const Real dir = sgn * xs;
+              const Real ds = dir + res;
+              const Real dira = sgn * xas;
+              const Real dsa = dira + res;
+              const Real isv = rcp_(sv), om = nu * isv;
+              const Real dna = -nu - om * dsa;
+              const Real dn = (sigma_mu - dsa * dna) * isv - nu - om * ds;
+              W.bs[10 * t + c] = sv + a * ds;
+              W.bnu[10 * t + c] = nu + a * dn;
+            };
+            row(0, R.u0h, -1, x.u0, xa.u0); row(1, R.u0l, 1, x.u0, xa.u0);
+            row(2, R.u1h, -1, x.u1, xa.u1); row(3, R.u1l, 1, x.u1, xa.u1);
+            if (N > 0) { row(4, R.dh, -1, x.d, xa.d); row(5, R.dl, 1, x.d, xa.d); }
+            if (t >= 1) {
+              row(6, R.r0h, -1, x.r0, xa.r0); row(7, R.r0l, 1, x.r0, xa.r0);
+              row(8, R.r1h, -1, x.r1, xa.r1); row(9, R.r1l, 1, x.r1, xa.r1);
+            }
           }
           if (acc) {
             const Real dx = W.s[3 * t + 3] - W.pref[2 * t], dy = W.s[3 * t + 4] - W.pref[2 * t + 1], dd = W.d[t];
