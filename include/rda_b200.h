@@ -315,6 +315,34 @@ int rda_convert_fleet_plan_obstacles(int B, int W, int N, int T, int E, float dt
                                      const float *fleet_plan_xy, float *obs_A, float *obs_b, int32_t *obs_kind,
                                      int32_t *obs_count, void *cuda_stream);
 
+/* HORIZON ORDER: rda_convert_world_obstacles / rda_convert_fleet_obstacles / rda_convert_fleet_plan_obstacles with each
+ * robot's shapes chosen by how close its horizon comes to them instead of the reference's sort key (DESIGN.md §7.3).
+ * The list is the same (the world's shapes, then, with a fleet, the map-mates in ascending index); shape j's key is
+ *   min over the finite pose columns q of nom_s[b][:, t] and ref_s[b][:, t], t = 0..T, of sd(body at q, shape j at t)
+ * where sd is rda_plan_clearance's signed distance and "shape j at t" the rows written for it (copy t when
+ * time_varying, copy 0 otherwise).  A column with a non-finite entry takes no part; without any, every key is +inf and
+ * the order is list order.  Stable ascending order, the first N, padding, obs_kind, obs_count and the rows are those of
+ * the calls above, and so are their arguments, except:
+ *   nom_s, ref_s [B][3][T+1]: the solver's nominal and reference poses (rda_pre_process_paths' outputs);
+ *   the robot body in the format of rda_fleet_shapes (body_kind RDA_OBS_POLYGON: body_nv counter-clockwise vertices
+ *   body_xy [body_nv][2], 3..8; RDA_OBS_CIRCLE: centre body_xy[0..1], body_radius > 0), or per robot body_xy_b
+ *   [B][RDA_MAX_EDGE][2] / body_radius_b [B] (device; NULL: the one body; values the caller's to check);
+ *   fleet_start NULL: no fleet, and the other fleet pointers are not read; fleet_plan_xy NULL: mates at constant
+ *   velocity, else along their plans (needs a fleet and time_varying).
+ * Usage errors are return codes: RDA_E_ARG for a NULL pointer or a bad body, RDA_E_UNSUPPORTED for N above
+ * RDA_MAX_WORLD_SLOTS, E outside 3..8 or a polygon body outside 3..8 vertices.  No allocation, host sync or graph break. */
+int rda_convert_world_obstacles_horizon(int B, int W, int N, int T, int E, float dt, int time_varying,
+                                        const float *nom_s, const float *ref_s, int body_kind, int body_nv,
+                                        const float *body_xy, float body_radius, const float *body_xy_b,
+                                        const float *body_radius_b, const int32_t *world_start,
+                                        const int32_t *robot_world, const int32_t *shape_kind, const int32_t *shape_nv,
+                                        const float *shape_xy, const float *shape_radius, const float *shape_vel,
+                                        const int32_t *fleet_start, const int32_t *fleet_robot,
+                                        const int32_t *fleet_kind, const int32_t *fleet_nv, const float *fleet_xy,
+                                        const float *fleet_radius, const float *fleet_vel, const float *fleet_plan_xy,
+                                        float *obs_A, float *obs_b, int32_t *obs_kind, int32_t *obs_count,
+                                        void *cuda_stream);
+
 /* Arrive rule of MPC.control (mpc.py:170-185, single gear): instances whose near_index >=
  * P - goal_index_threshold get u_opt = 0 and arrive = 1; cur_vel (may be NULL) receives the
  * controls kept as the next step's nominal (mpc.py:186).  u_opt, cur_vel [B][2][T].        */

@@ -62,7 +62,8 @@ EXPORTS = ['rda_create', 'rda_destroy', 'rda_set_tunables', 'rda_get_tunables', 
            'rda_pre_process_paths', 'rda_post_process_paths', 'rda_fleet_shapes', 'rda_convert_fleet_obstacles',
            'rda_set_instance_params', 'rda_set_robot_classes', 'rda_set_robot_class_index',
            'rda_pre_process_paths_per_robot', 'rda_motion_predict_per_robot', 'rda_fleet_shapes_per_robot',
-           'rda_plan_clearance', 'rda_fleet_plan_shapes', 'rda_convert_fleet_plan_obstacles']
+           'rda_plan_clearance', 'rda_fleet_plan_shapes', 'rda_convert_fleet_plan_obstacles',
+           'rda_convert_world_obstacles_horizon']
 MAX_SHAPES = 64
 MAX_WORLD_SLOTS = 256
 
@@ -119,6 +120,7 @@ def load():
     lib.rda_convert_fleet_obstacles.argtypes = [i, i, i, i, i, f, i, i] + [vp] * 20
     lib.rda_fleet_plan_shapes.argtypes = [i, i, i, f, f, i, i, vp, f] + [vp] * 13
     lib.rda_convert_fleet_plan_obstacles.argtypes = [i, i, i, i, i, f, i, i] + [vp] * 21
+    lib.rda_convert_world_obstacles_horizon.argtypes = [i, i, i, i, i, f, i, vp, vp, i, i, vp, f] + [vp] * 22
     for name in EXPORTS:
         if name != 'rda_version':
             getattr(lib, name).restype = C.c_int

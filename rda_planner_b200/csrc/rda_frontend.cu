@@ -8,6 +8,7 @@
 #include "../../include/rda_b200.h"
 #include "rda_hd.h"
 #include "frontend.cuh"
+#include "horizon_key.cuh"
 
 using namespace rda;
 
@@ -129,6 +130,75 @@ __device__ __forceinline__ size_t list_entry(const ShapeList& L, int i, const in
   return (size_t)(m < 0 ? 0 : (m >= B ? B - 1 : m));   // a malformed list never reads outside the fleet
 }
 
+// The candidates of a tile, c (ckey, cidx) pairs in any order, ranked among themselves into (skey, sidx) and merged with
+// the nk kept pairs of buffer cur into buffer cur ^ 1, the first N kept.  Every element's new position is its rank in
+// its own list plus its rank in the other.  Ends with a barrier of the CTA.
+__device__ __forceinline__ void world_merge(int tid, int c, int N, double* kkey, int* kidx, const double* ckey,
+                                            const int* cidx, double* skey, int* sidx, int& nk, int& cur) {
+  if (tid < c) {                                       // rank among the candidates: sorted copy
+    const double k = ckey[tid];
+    const int ix = cidx[tid];
+    int r = 0;
+    for (int j = 0; j < c; ++j) r += obstacle_before(ckey[j], cidx[j], k, ix);
+    skey[r] = k; sidx[r] = ix;
+  }
+  __syncthreads();
+  const int nxt = cur ^ 1;
+  const double* ok = kkey + cur * N;
+  const int* oi = kidx + cur * N;
+  if (tid < c) {
+    const int p = tid + world_rank(ok, oi, nk, skey[tid], sidx[tid]);
+    if (p < N) { kkey[nxt * N + p] = skey[tid]; kidx[nxt * N + p] = sidx[tid]; }
+  }
+  for (int j = tid; j < nk; j += kWorldTile) {
+    const int p = j + world_rank(skey, sidx, c, ok[j], oi[j]);
+    if (p < N) { kkey[nxt * N + p] = ok[j]; kidx[nxt * N + p] = oi[j]; }
+  }
+  nk = nk + c < N ? nk + c : N;
+  cur = nxt;
+  __syncthreads();
+}
+
+// The rows of the N slots of robot b: slot n is the list entry kept_idx[n] (list order when kept_idx is NULL), the
+// last one repeated past the list, all-zero rows for an empty list.  kPlan: map-mates are read along fleet_plan_xy.
+template <bool kPlan>
+__device__ __forceinline__ void world_slots(int tid, int b, int B, int N, int T, int E, float dt, int time_varying,
+                                            int count, const ShapeList& L, const int* kept_idx, const int* shape_kind,
+                                            const int* shape_nv, const float* shape_xy, const float* shape_radius,
+                                            const float* shape_vel, const int* fleet_robot, const int* fleet_kind,
+                                            const int* fleet_nv, const float* fleet_xy, const float* fleet_radius,
+                                            const float* fleet_vel, const float* fleet_plan_xy, float* obs_A,
+                                            float* obs_b, int* obs_kind) {
+  const int Tc = time_varying ? T + 1 : 1;
+  for (int q = tid; q < N * Tc; q += kWorldTile) {     // one (slot, stage) copy per thread
+    const int n = q / Tc, t = q - n * Tc;
+    float* A = obs_A + (((size_t)b * N + n) * Tc + t) * E * 2;
+    float* bb = obs_b + (((size_t)b * N + n) * Tc + t) * E;
+    if (count == 0) {
+      for (int r = 0; r < E; ++r) { A[2 * r] = 0.f; A[2 * r + 1] = 0.f; bb[r] = 0.f; }
+      if (t == 0) obs_kind[(size_t)b * N + n] = RDA_OBS_POLYGON;
+      continue;
+    }
+    const int slot = n < count ? n : count - 1;        // pad by repeating the last
+    int src = kept_idx ? kept_idx[slot] : slot;
+    if (src < 0 || src >= count) src = count - 1;      // NaN keys have no order; never read outside the list
+    bool mate;
+    const size_t s = list_entry(L, src, fleet_robot, b, B, &mate);
+    const int kind = (mate ? fleet_kind : shape_kind)[s];
+    if (t == 0) obs_kind[(size_t)b * N + n] = kind;
+    const float* xy = (mate ? fleet_xy : shape_xy) + s * RDA_MAX_EDGE * 2;
+    double vx = 0.0, vy = 0.0;
+    if (kPlan && mate) {                               // a map-mate along its plan: its stage-t shape, standing
+      xy = fleet_plan_xy + (s * (T + 1) + t) * RDA_MAX_EDGE * 2;
+    } else {
+      const float* vel = (mate ? fleet_vel : shape_vel) + 2 * s;
+      vx = vel[0]; vy = vel[1];
+    }
+    obstacle_rows(kind, (mate ? fleet_nv : shape_nv)[s], xy, (mate ? fleet_radius : shape_radius)[s], vx, vy, t,
+                  (double)dt, E, A, bb);
+  }
+}
+
 // kPlan: map-mates are read along their plans, fleet_plan_xy [B][T+1][RDA_MAX_EDGE][2] (time-varying output only);
 // the variant without plans never reads it, and compiles to the code it had before plans existed.
 template <bool kPlan>
@@ -190,60 +260,139 @@ k_convert_world_obstacles(int B, int W, int N, int T, int E, float dt, int time_
       __syncthreads();
       const int c = n_cand[tile];
       if (c == 0) continue;
-      if (tid < c) {                                   // rank among the candidates: sorted copy
-        const double k = ckey[tid];
-        const int ix = cidx[tid];
-        int r = 0;
-        for (int j = 0; j < c; ++j) r += obstacle_before(ckey[j], cidx[j], k, ix);
-        skey[r] = k; sidx[r] = ix;
-      }
-      __syncthreads();
-      const int nxt = cur ^ 1;
-      const double* ok = kkey + cur * N;
-      const int* oi = kidx + cur * N;
-      if (tid < c) {
-        const int p = tid + world_rank(ok, oi, nk, skey[tid], sidx[tid]);
-        if (p < N) { kkey[nxt * N + p] = skey[tid]; kidx[nxt * N + p] = sidx[tid]; }
-      }
-      for (int j = tid; j < nk; j += kWorldTile) {
-        const int p = j + world_rank(skey, sidx, c, ok[j], oi[j]);
-        if (p < N) { kkey[nxt * N + p] = ok[j]; kidx[nxt * N + p] = oi[j]; }
-      }
-      nk = nk + c < N ? nk + c : N;
-      cur = nxt;
-      __syncthreads();
+      world_merge(tid, c, N, kkey, kidx, ckey, cidx, skey, sidx, nk, cur);
     }
     kept_idx = kidx + cur * N;
   }
   if (tid == 0) obs_count[b] = count;
-  const int Tc = time_varying ? T + 1 : 1;
-  for (int q = tid; q < N * Tc; q += kWorldTile) {     // one (slot, stage) copy per thread
-    const int n = q / Tc, t = q - n * Tc;
-    float* A = obs_A + (((size_t)b * N + n) * Tc + t) * E * 2;
-    float* bb = obs_b + (((size_t)b * N + n) * Tc + t) * E;
-    if (count == 0) {
-      for (int r = 0; r < E; ++r) { A[2 * r] = 0.f; A[2 * r + 1] = 0.f; bb[r] = 0.f; }
-      if (t == 0) obs_kind[(size_t)b * N + n] = RDA_OBS_POLYGON;
-      continue;
+  world_slots<kPlan>(tid, b, B, N, T, E, dt, time_varying, count, L, kept_idx, shape_kind, shape_nv, shape_xy,
+                     shape_radius, shape_vel, fleet_robot, fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel,
+                     fleet_plan_xy, obs_A, obs_b, obs_kind);
+}
+
+// Horizon order (rda_convert_world_obstacles_horizon): the tiles, candidates and merge of k_convert_world_obstacles
+// with the key of horizon_key.cuh, the smallest signed distance of the robot's body over its nominal and reference
+// poses.  Each tile goes in three steps:
+//  1. a thread per shape: once N pairs are kept, a shape whose lower bound (the one-disc bound of the whole horizon,
+//     then the bound of every pose) is >= the N-th kept key cannot enter, as every later shape has a larger index and
+//     loses ties; the others are listed as survivors;
+//  2. a warp per survivor: one lane per pose (2 (T + 1) poses), each the stage shape's rows and plan_clearance_cell,
+//     and the warp's minimum: the exact key; keys that beat the N-th become candidates;
+//  3. the merge of k_convert_world_obstacles.
+// The selection is therefore that of sorting every exact key.  EC / RC: compile-time caps of the obstacle rows and
+// body vertices (plan_clearance_cell).  The body (the one body, or body_xy_b [b] / body_radius_b [b]) and the horizon
+// disc are staged once in shared memory.
+template <int EC, int RC, bool kPlan>
+__global__ void __launch_bounds__(kWorldTile)
+k_convert_world_obstacles_horizon(int B, int W, int N, int T, int E, float dt, int time_varying, const float* nom_s,
+                                  const float* ref_s, int body_kind, int body_nv, const float* body_xy,
+                                  float body_radius, const float* body_xy_b, const float* body_radius_b,
+                                  const int* world_start, const int* robot_world, const int* shape_kind,
+                                  const int* shape_nv, const float* shape_xy, const float* shape_radius,
+                                  const float* shape_vel, const int* fleet_start, const int* fleet_robot,
+                                  const int* fleet_kind, const int* fleet_nv, const float* fleet_xy,
+                                  const float* fleet_radius, const float* fleet_vel, const float* fleet_plan_xy,
+                                  float* obs_A, float* obs_b, int* obs_kind, int* obs_count) {
+  // dynamic shared memory: as k_convert_world_obstacles, then the survivors of a tile [tile]
+  extern __shared__ double sh[];
+  __shared__ int n_surv, n_cand;
+  __shared__ RobotGeom body;
+  __shared__ double hor[4];                            // horizon disc centre, radius; body reach
+  const int b = blockIdx.x;
+  if (b >= B) return;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int w = robot_world ? robot_world[b] : 0;
+  ShapeList L = {0, 0, 0, 0};
+  if (w >= 0 && w < W) {
+    L.first = world_start[w];
+    L.n_world = world_start[w + 1] - L.first;
+    if (L.n_world < 0) L.n_world = 0;
+    if (fleet_start) {
+      L.mate0 = fleet_start[w];
+      L.mates = fleet_start[w + 1] - L.mate0 - 1;
+      if (L.mates < 0) L.mates = 0;
     }
-    const int slot = n < count ? n : count - 1;        // pad by repeating the last
-    int src = kept_idx ? kept_idx[slot] : slot;
-    if (src < 0 || src >= count) src = count - 1;      // NaN keys have no order; never read outside the list
-    bool mate;
-    const size_t s = list_entry(L, src, fleet_robot, b, B, &mate);
-    const int kind = (mate ? fleet_kind : shape_kind)[s];
-    if (t == 0) obs_kind[(size_t)b * N + n] = kind;
-    const float* xy = (mate ? fleet_xy : shape_xy) + s * RDA_MAX_EDGE * 2;
-    double vx = 0.0, vy = 0.0;
-    if (kPlan && mate) {                               // a map-mate along its plan: its stage-t shape, standing
-      xy = fleet_plan_xy + (s * (T + 1) + t) * RDA_MAX_EDGE * 2;
-    } else {
-      const float* vel = (mate ? fleet_vel : shape_vel) + 2 * s;
-      vx = vel[0]; vy = vel[1];
-    }
-    obstacle_rows(kind, (mate ? fleet_nv : shape_nv)[s], xy, (mate ? fleet_radius : shape_radius)[s], vx, vy, t,
-                  (double)dt, E, A, bb);
   }
+  const int count = L.n_world + L.mates;
+  const int T1 = T + 1;
+  const double dtd = dt;
+  int cur = 0;
+  int* kept_idx = nullptr;
+  if (count > 0) {
+    double* kkey = sh;                                 // [2][N]
+    double* ckey = kkey + 2 * N;                       // gathered [tile], sorted [tile]
+    double* skey = ckey + kWorldTile;
+    int* kidx = (int*)(skey + kWorldTile);             // [2][N]
+    int* cidx = kidx + 2 * N;
+    int* sidx = cidx + kWorldTile;
+    int* surv = sidx + kWorldTile;                     // [tile]
+    const float* nom = nom_s + (size_t)b * 3 * T1;
+    const float* ref = ref_s + (size_t)b * 3 * T1;
+    if (tid == 0) {
+      body_geom(body_kind, body_nv, body_xy_b ? body_xy_b + (size_t)b * RDA_MAX_EDGE * 2 : body_xy,
+                body_radius_b ? body_radius_b[b] : body_radius, &body);
+      hor[3] = body_reach(body);
+      if (horizon_disc(nom, ref, T, &hor[0], &hor[1], &hor[2]) == 0) hor[2] = -1;   // no finite pose: keys +inf
+    }
+    int nk = 0;                                        // pairs kept so far (uniform across the CTA)
+    for (int base = 0; base < count; base += kWorldTile) {
+      if (tid == 0) { n_surv = 0; n_cand = 0; }
+      __syncthreads();                                 // also: the previous tile's counters have been read
+      const double thr = nk < N ? INFINITY : kkey[cur * N + N - 1];
+      const int i = base + tid;
+      if (i < count) {
+        bool mate;
+        const size_t s = list_entry(L, i, fleet_robot, b, B, &mate);
+        bool keep = nk < N;
+        if (!keep && hor[2] >= 0) {                    // without a finite pose every key is +inf and loses to the kept
+          const float* vel = (mate ? fleet_vel : shape_vel) + 2 * s;
+          const RawShape r = {(mate ? fleet_kind : shape_kind)[s], (mate ? fleet_nv : shape_nv)[s],
+                              (mate ? fleet_xy : shape_xy) + s * RDA_MAX_EDGE * 2,
+                              (double)(mate ? fleet_radius : shape_radius)[s], (double)vel[0], (double)vel[1],
+                              kPlan && mate ? fleet_plan_xy + s * T1 * RDA_MAX_EDGE * 2 : nullptr};
+          keep = horizon_disc_bound(r, time_varying, T, dtd, E, hor[0], hor[1], hor[2], hor[3]) < thr &&
+                 horizon_bound(r, time_varying, T, dtd, E, nom, ref, hor[3], thr) < thr;
+        }
+        if (keep) surv[atomicAdd(&n_surv, 1)] = i;
+      }
+      __syncthreads();
+      const int ns = n_surv;
+      for (int k = warp; k < ns; k += kWorldTile / 32) {   // a warp per survivor, a lane per pose
+        const int ix = surv[k];
+        bool mate;
+        const size_t s = list_entry(L, ix, fleet_robot, b, B, &mate);
+        const float* vel = (mate ? fleet_vel : shape_vel) + 2 * s;
+        const RawShape r = {(mate ? fleet_kind : shape_kind)[s], (mate ? fleet_nv : shape_nv)[s],
+                            (mate ? fleet_xy : shape_xy) + s * RDA_MAX_EDGE * 2,
+                            (double)(mate ? fleet_radius : shape_radius)[s], (double)vel[0], (double)vel[1],
+                            kPlan && mate ? fleet_plan_xy + s * T1 * RDA_MAX_EDGE * 2 : nullptr};
+        double key = INFINITY;
+        for (int q = lane; q < 2 * T1; q += 32) {
+          const float* p = q < T1 ? nom : ref;
+          const int t = q < T1 ? q : q - T1;
+          if (!pose_finite(p, T1, t)) continue;
+          const double v = horizon_cell<EC, RC>(body, r, time_varying ? t : 0, dtd, E, p[t], p[T1 + t], p[2 * T1 + t]);
+          if (v < key) key = v;
+        }
+        for (int off = 16; off > 0; off >>= 1) {
+          const double o = __shfl_xor_sync(0xffffffffu, key, off);
+          key = o < key ? o : key;
+        }
+        if (lane == 0 && (nk < N || key < thr)) {
+          const int p = atomicAdd(&n_cand, 1);
+          ckey[p] = key; cidx[p] = ix;
+        }
+      }
+      __syncthreads();
+      const int c = n_cand;
+      if (c > 0) world_merge(tid, c, N, kkey, kidx, ckey, cidx, skey, sidx, nk, cur);
+    }
+    kept_idx = kidx + cur * N;
+  }
+  if (tid == 0) obs_count[b] = count;
+  world_slots<kPlan>(tid, b, B, N, T, E, dt, time_varying, count, L, kept_idx, shape_kind, shape_nv, shape_xy,
+                     shape_radius, shape_vel, fleet_robot, fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel,
+                     fleet_plan_xy, obs_A, obs_b, obs_kind);
 }
 
 // Each robot of a fleet as a raw shape for its map-mates (fleet_shape), one thread per robot: its body at its pose,
@@ -337,6 +486,45 @@ int launch_world_obstacles(bool fleet, int B, int W, int N, int T, int E, float 
       B, W, N, T, E, dt, time_varying, order, state, world_start, robot_world, shape_kind, shape_nv, shape_xy,
       shape_radius, shape_vel, fleet_start, fleet_robot, fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel,
       fleet_plan_xy, obs_A, obs_b, obs_kind, obs_count);
+  RDA_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// Argument checks and launch of k_convert_world_obstacles_horizon.  fleet_start NULL: no fleet (the other fleet
+// pointers are then not read); fleet_plan_xy (fleet only, time-varying output only) may be NULL.
+int launch_world_obstacles_horizon(int B, int W, int N, int T, int E, float dt, int time_varying, const float* nom_s,
+                                   const float* ref_s, int body_kind, int body_nv, const float* body_xy,
+                                   float body_radius, const float* body_xy_b, const float* body_radius_b,
+                                   const int32_t* world_start, const int32_t* robot_world, const int32_t* shape_kind,
+                                   const int32_t* shape_nv, const float* shape_xy, const float* shape_radius,
+                                   const float* shape_vel, const int32_t* fleet_start, const int32_t* fleet_robot,
+                                   const int32_t* fleet_kind, const int32_t* fleet_nv, const float* fleet_xy,
+                                   const float* fleet_radius, const float* fleet_vel, const float* fleet_plan_xy,
+                                   float* obs_A, float* obs_b, int32_t* obs_kind, int32_t* obs_count,
+                                   cudaStream_t stream) {
+  if (B < 1 || W < 1 || N < 1 || T < 1) return RDA_E_ARG;
+  if (N > RDA_MAX_WORLD_SLOTS || E < 3 || E > RDA_MAX_EDGE) return RDA_E_UNSUPPORTED;
+  if (body_kind == RDA_OBS_POLYGON) {
+    if (body_nv < 3 || body_nv > RDA_MAX_ROBOT_EDGE) return RDA_E_UNSUPPORTED;
+  } else if (body_kind != RDA_OBS_CIRCLE || (!body_radius_b && !(body_radius > 0.f))) {
+    return RDA_E_ARG;
+  }
+  if ((!body_xy && !body_xy_b) || !nom_s || !ref_s) return RDA_E_ARG;
+  if (!world_start || !shape_kind || !shape_nv || !shape_xy || !shape_radius || !shape_vel) return RDA_E_ARG;
+  if (!obs_A || !obs_b || !obs_kind || !obs_count) return RDA_E_ARG;
+  const bool fleet = fleet_start != nullptr;
+  if (fleet && (!fleet_robot || !fleet_kind || !fleet_nv || !fleet_xy || !fleet_radius || !fleet_vel)) return RDA_E_ARG;
+  if (fleet_plan_xy && (!fleet || !time_varying)) return RDA_E_ARG;
+  const bool small = E <= 4 && (body_kind == RDA_OBS_CIRCLE || body_nv <= 4);
+  const bool plan = fleet_plan_xy != nullptr;
+  auto k = small ? (plan ? k_convert_world_obstacles_horizon<4, 4, true> : k_convert_world_obstacles_horizon<4, 4, false>)
+                 : (plan ? k_convert_world_obstacles_horizon<8, 8, true> : k_convert_world_obstacles_horizon<8, 8, false>);
+  const size_t smem = (size_t)(2 * N + 2 * kWorldTile) * (sizeof(double) + sizeof(int)) + kWorldTile * sizeof(int);
+  k<<<B, kWorldTile, smem, stream>>>(B, W, N, T, E, dt, time_varying, nom_s, ref_s, body_kind, body_nv, body_xy,
+                                     body_radius, body_xy_b, body_radius_b, world_start, robot_world, shape_kind,
+                                     shape_nv, shape_xy, shape_radius, shape_vel, fleet_start, fleet_robot, fleet_kind,
+                                     fleet_nv, fleet_xy, fleet_radius, fleet_vel, fleet_plan_xy, obs_A, obs_b, obs_kind,
+                                     obs_count);
   RDA_CUDA(cudaGetLastError());
   return 0;
 }
@@ -535,6 +723,24 @@ int rda_convert_fleet_plan_obstacles(int B, int W, int N, int T, int E, float dt
                                 shape_kind, shape_nv, shape_xy, shape_radius, shape_vel, fleet_start, fleet_robot,
                                 fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel, fleet_plan_xy, obs_A, obs_b,
                                 obs_kind, obs_count, (cudaStream_t)stream);
+}
+
+int rda_convert_world_obstacles_horizon(int B, int W, int N, int T, int E, float dt, int time_varying,
+                                        const float* nom_s, const float* ref_s, int body_kind, int body_nv,
+                                        const float* body_xy, float body_radius, const float* body_xy_b,
+                                        const float* body_radius_b, const int32_t* world_start,
+                                        const int32_t* robot_world, const int32_t* shape_kind, const int32_t* shape_nv,
+                                        const float* shape_xy, const float* shape_radius, const float* shape_vel,
+                                        const int32_t* fleet_start, const int32_t* fleet_robot,
+                                        const int32_t* fleet_kind, const int32_t* fleet_nv, const float* fleet_xy,
+                                        const float* fleet_radius, const float* fleet_vel, const float* fleet_plan_xy,
+                                        float* obs_A, float* obs_b, int32_t* obs_kind, int32_t* obs_count,
+                                        void* stream) {
+  return launch_world_obstacles_horizon(B, W, N, T, E, dt, time_varying, nom_s, ref_s, body_kind, body_nv, body_xy,
+                                        body_radius, body_xy_b, body_radius_b, world_start, robot_world, shape_kind,
+                                        shape_nv, shape_xy, shape_radius, shape_vel, fleet_start, fleet_robot,
+                                        fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel, fleet_plan_xy, obs_A,
+                                        obs_b, obs_kind, obs_count, (cudaStream_t)stream);
 }
 
 int rda_post_process(int B, int T, int P, int goal_index_threshold, const int32_t* near_index, float* u_opt,

@@ -9,6 +9,9 @@
   fleet_shapes_batch, convert_fleet_obstacles_batch
                            the same with the other robots of each world as moving obstacles
   fleet_plan_shapes_batch  the robots along their last plans, for convert_fleet_obstacles_batch(plan=True)
+  convert_world_obstacles_horizon_batch
+                           the world and fleet conversions in the horizon order: each robot's shapes sorted by the
+                           smallest signed distance of its body over its nominal and reference poses
   pack_paths               a set of reference paths cut into single-gear curves (split_path, mpc.py:232-249),
                            in the layout the device reads
   BatchedMPC               MPC.control for B robots, on one reference path or each on its own path of a
@@ -327,6 +330,40 @@ def convert_fleet_obstacles_batch(world, state, robot_world, fleet, N, T, E, dt,
     return A, b, kind, count
 
 
+def convert_world_obstacles_horizon_batch(world, nom_s, ref_s, body, robot_world, N, T, E, dt, time_varying=False,
+                                          fleet=None, plan=False, per_robot=None):
+    """convert_world_obstacles_batch (fleet None) or convert_fleet_obstacles_batch (fleet from fleet_shapes_batch or,
+    with plan, fleet_plan_shapes_batch) in the horizon order: each robot's shapes sorted by the smallest signed distance
+    between its body and the shape's rows over its nominal and reference poses, nom_s, ref_s [B,3,T+1] CUDA tensors.
+    body from robot_body with xy a CUDA tensor; per_robot None, or a dict with CUDA tensors 'xy' [B,8,2] and 'radius'
+    [B], each robot's own body (body gives the kind and vertex count).  The same list, padding, outputs and obs_count
+    as those calls; without a host synchronisation."""
+    if plan and (fleet is None or not time_varying):
+        raise ValueError('a fleet predicted along its plans needs a fleet and time_varying=True')
+    lib = _cabi.load()
+    dev = nom_s.device
+    B, W = nom_s.shape[0], world['start'].shape[0] - 1
+    Tc = T + 1 if time_varying else 1
+    A = torch.empty((B, N, Tc, E, 2), dtype=torch.float32, device=dev)
+    b = torch.empty((B, N, Tc, E), dtype=torch.float32, device=dev)
+    kind = torch.empty((B, N), dtype=torch.int32, device=dev)
+    count = torch.empty(B, dtype=torch.int32, device=dev)
+    mates = (None,) * 8
+    if fleet is not None:
+        csr = fleet_csr(robot_world if robot_world is not None else torch.zeros(B, dtype=torch.int32, device=dev), W)
+        mates = (_ptr(csr[0]), _ptr(csr[1]), _ptr(fleet['kind']), _ptr(fleet['nv']), _ptr(fleet['xy']),
+                 _ptr(fleet['radius']), _ptr(fleet['vel']), _ptr(fleet['plan_xy']) if plan else None)
+    pr = per_robot or {}
+    with torch.cuda.device(dev):
+        _cabi.check(lib.rda_convert_world_obstacles_horizon(
+            B, W, N, T, E, dt, int(time_varying), _ptr(nom_s), _ptr(ref_s), int(body['kind']), int(body['nv']),
+            _ptr(body['xy']), float(body['radius']), _ptr(pr.get('xy')), _ptr(pr.get('radius')), _ptr(world['start']),
+            _ptr(robot_world), _ptr(world['kind']), _ptr(world['nv']), _ptr(world['xy']), _ptr(world['radius']),
+            _ptr(world['vel']), *mates, _ptr(A), _ptr(b), _ptr(kind), _ptr(count), _stream(dev)),
+            'rda_convert_world_obstacles_horizon')
+    return A, b, kind, count
+
+
 def shapes_to_device(shapes, device):
     return {k: torch.as_tensor(v, device=device).contiguous() for k, v in shapes.items()}
 
@@ -355,7 +392,13 @@ class BatchedMPC:
     With `robot_class` [B], car_tuple is a list of up to 16 car_tuples (robot classes of one cone_type and one number of
     canonical body rows) and robot b is of class robot_class[b]: its body, wheelbase, dynamics and limits (and its body
     and motion as others see it with avoid_fleet).  The handle is built with class 0, so an index outside the list means
-    class 0.  set_robot_class moves robots between classes on the device."""
+    class 0.  set_robot_class moves robots between classes on the device.
+
+    obstacle_order: True sorts each robot's obstacles by the reference's key (mpc.py:210-218, the distance from its
+    position to a polygon's nearest vertex or a disc's centre), False keeps list order, and 'horizon' sorts them by how
+    close the robot's horizon comes to them: the smallest signed distance between its body and the obstacle's rows over
+    its nominal and reference poses (convert_world_obstacles_horizon_batch).  'horizon' takes world= (and avoid_fleet),
+    not shapes=."""
 
     def __init__(self, car_tuple, ref_path, batch, receding=10, sample_time=0.1, iter_num=4,
                  enable_reverse=False, obstacle_order=True, max_edge_num=5, max_obs_num=5,
@@ -369,6 +412,8 @@ class BatchedMPC:
             if not self.classes:
                 raise ValueError('robot_class needs at least one car_tuple')
             car_tuple = self.classes[0]
+        if isinstance(obstacle_order, str) and obstacle_order != 'horizon':
+            raise ValueError(f"obstacle_order is True, False or 'horizon', not {obstacle_order!r}")
         self.rda = RDA_solver(receding, car_tuple, max_edge_num, max_obs_num, iter_num=iter_num,
                               step_time=sample_time, iter_threshold=iter_threshold, accelerated=accelerated,
                               time_print=False, batch=batch, device=device, **kwargs)
@@ -491,6 +536,10 @@ class BatchedMPC:
             raise ValueError("fleet_prediction='plan' predicts the map-mates of avoid_fleet=True")
         if plan and not time_varying:
             raise ValueError("fleet_prediction='plan' needs time_varying=True: the prediction is a trajectory")
+        horizon = isinstance(self.obstacle_order, str)
+        if horizon and shapes is not None:
+            raise ValueError("obstacle_order='horizon' selects from worlds, not from shapes=: pass the lists as worlds "
+                             "(world=pack_worlds(lists), one world per robot, robot_world=arange(B))")
         if avoid_fleet:
             if shapes is not None:
                 raise ValueError('avoid_fleet takes its obstacles from world= (or an empty map), not from shapes')
@@ -534,6 +583,15 @@ class BatchedMPC:
         if (shapes is None and world is None) or self.N == 0:
             A, b, kind, count = self._no_obstacles()
             time_varying = False
+        elif horizon:
+            fleet = None
+            if avoid_fleet:
+                fleet = fleet_shapes_batch(state, self.cur_vel, self.body, self.dynamics, self.per_robot) if not plan \
+                    else fleet_plan_shapes_batch(state, self.cur_vel, self.body, self.dynamics, self.dt, self.L,
+                                                 self.per_robot)
+            A, b, kind, count = convert_world_obstacles_horizon_batch(world, nom_s, ref_s, self.body, robot_world, self.N,
+                                                                      T, self.E, self.dt, time_varying, fleet, plan,
+                                                                      self.per_robot)
         elif avoid_fleet:
             if plan:
                 fleet = fleet_plan_shapes_batch(state, self.cur_vel, self.body, self.dynamics, self.dt, self.L,
