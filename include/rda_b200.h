@@ -135,6 +135,21 @@ int rda_set_robot_classes(rda_handle *h, int K, const rda_robot_class *classes, 
  * wheelbase and dynamics (decided on the device).  robot_class = NULL: the handle's own for every instance.
  * rda_reset and rda_cold_start leave the classes and the index alone. */
 int rda_set_robot_class_index(rda_handle *h, const int32_t *robot_class, void *cuda_stream);
+/* Warm start that follows the obstacles (DESIGN.md §7.4).  The front ends choose each instance's obstacles again at every
+ * step, so slot n holds whichever obstacle ranks n; by default (as in the reference, assign_obstacle_parameter :483-526)
+ * the warm-start state stays in its slot.  obs_id: DEVICE pointer to int32 [B][N], the obstacle that slot n of instance b
+ * holds in the next solve (the rda_convert_*_ids calls write them; values < 0: no obstacle, never matched).  When the
+ * handle holds the ids of an earlier call, each instance's per-slot state moves with its obstacles: the k-th slot (in
+ * slot order) carrying id X takes the state of the k-th slot that carried X, so the padding copies of a repeated last
+ * obstacle match copy to copy; a slot without a match gets the values rda_cold_start writes.  The moved state is
+ * everything indexed by slot that a solve leaves behind: RDA_BUF_LAM, MU, Z, XI, ZETA, all five planes of COEF, and the
+ * coherent pass's support-vertex hints; per-instance state (DIS, PREF, CUR_S, CUR_U, status) stays.  Then the handle
+ * keeps obs_id for the next call.  The first call after rda_create or after obs_id = NULL only stores the ids; NULL
+ * forgets them (back to the slot behaviour).  rda_reset and rda_cold_start keep the ids.  One kernel on cuda_stream
+ * for the whole batch (none when storing), no host synchronisation, no allocation after the first call (the id storage),
+ * CUDA-graph capturable (whether a call stores or moves is decided on the host and fixed in a captured graph); not
+ * counted in rda_last_launch_count.  RDA_E_UNSUPPORTED for N above 4096 (the kernel's ids in 48 KB of shared memory). */
+int rda_set_obstacle_ids(rda_handle *h, const int32_t *obs_id, void *cuda_stream);
 /* RDA_solver.reset (:1060-1068): clears lam'A and lam'b only. */
 int rda_reset(rda_handle *h, void *cuda_stream);
 /* Clear ALL warm-start state back to the constructor values (extension; used by benchmarks). */
@@ -342,6 +357,41 @@ int rda_convert_world_obstacles_horizon(int B, int W, int N, int T, int E, float
                                         const float *fleet_radius, const float *fleet_vel, const float *fleet_plan_xy,
                                         float *obs_A, float *obs_b, int32_t *obs_kind, int32_t *obs_count,
                                         void *cuda_stream);
+
+/* The conversions above that also say which obstacle went where, for rda_set_obstacle_ids: obs_A, obs_b, obs_kind and
+ * obs_count are those of the existing call, bit for bit, and obs_id [B][N] (device) receives each slot's obstacle id:
+ *   rda_convert_obstacles_ids: the position j of the shape in the robot's list (shape_kind[b][j] ...);
+ *   rda_convert_world_obstacles_ids: the arguments of rda_convert_fleet_plan_obstacles, where fleet_start = NULL means a
+ *     world only (the other fleet pointers are then not read) and fleet_plan_xy = NULL mates at constant velocity; the id
+ *     is the flat shape index s for a world shape and world_start[W] + m for map-mate robot m;
+ *   rda_convert_world_obstacles_horizon_ids: rda_convert_world_obstacles_horizon, with the same ids.
+ * A robot with an empty list gets -1 in every slot.  Identity is list position: a caller who repacks a map must keep its
+ * order for the warm start to follow.  Usage errors as the existing calls, and RDA_E_ARG for obs_id = NULL. */
+int rda_convert_obstacles_ids(int B, int M, int N, int T, int E, float dt, int time_varying, int order,
+                              const float *state, const int32_t *shape_kind, const int32_t *shape_nv,
+                              const float *shape_xy, const float *shape_radius, const float *shape_vel,
+                              const int32_t *shape_count, float *obs_A, float *obs_b, int32_t *obs_kind,
+                              int32_t *obs_count, int32_t *obs_id, void *cuda_stream);
+int rda_convert_world_obstacles_ids(int B, int W, int N, int T, int E, float dt, int time_varying, int order,
+                                    const float *state, const int32_t *world_start, const int32_t *robot_world,
+                                    const int32_t *shape_kind, const int32_t *shape_nv, const float *shape_xy,
+                                    const float *shape_radius, const float *shape_vel, const int32_t *fleet_start,
+                                    const int32_t *fleet_robot, const int32_t *fleet_kind, const int32_t *fleet_nv,
+                                    const float *fleet_xy, const float *fleet_radius, const float *fleet_vel,
+                                    const float *fleet_plan_xy, float *obs_A, float *obs_b, int32_t *obs_kind,
+                                    int32_t *obs_count, int32_t *obs_id, void *cuda_stream);
+int rda_convert_world_obstacles_horizon_ids(int B, int W, int N, int T, int E, float dt, int time_varying,
+                                            const float *nom_s, const float *ref_s, int body_kind, int body_nv,
+                                            const float *body_xy, float body_radius, const float *body_xy_b,
+                                            const float *body_radius_b, const int32_t *world_start,
+                                            const int32_t *robot_world, const int32_t *shape_kind,
+                                            const int32_t *shape_nv, const float *shape_xy, const float *shape_radius,
+                                            const float *shape_vel, const int32_t *fleet_start,
+                                            const int32_t *fleet_robot, const int32_t *fleet_kind,
+                                            const int32_t *fleet_nv, const float *fleet_xy, const float *fleet_radius,
+                                            const float *fleet_vel, const float *fleet_plan_xy, float *obs_A,
+                                            float *obs_b, int32_t *obs_kind, int32_t *obs_count, int32_t *obs_id,
+                                            void *cuda_stream);
 
 /* Arrive rule of MPC.control (mpc.py:170-185, single gear): instances whose near_index >=
  * P - goal_index_threshold get u_opt = 0 and arrive = 1; cur_vel (may be NULL) receives the

@@ -63,7 +63,8 @@ EXPORTS = ['rda_create', 'rda_destroy', 'rda_set_tunables', 'rda_get_tunables', 
            'rda_set_instance_params', 'rda_set_robot_classes', 'rda_set_robot_class_index',
            'rda_pre_process_paths_per_robot', 'rda_motion_predict_per_robot', 'rda_fleet_shapes_per_robot',
            'rda_plan_clearance', 'rda_fleet_plan_shapes', 'rda_convert_fleet_plan_obstacles',
-           'rda_convert_world_obstacles_horizon']
+           'rda_convert_world_obstacles_horizon', 'rda_set_obstacle_ids', 'rda_convert_obstacles_ids',
+           'rda_convert_world_obstacles_ids', 'rda_convert_world_obstacles_horizon_ids']
 MAX_SHAPES = 64
 MAX_WORLD_SLOTS = 256
 
@@ -89,6 +90,7 @@ def load():
     lib.rda_set_instance_params.argtypes = [vp, vp, vp]
     lib.rda_set_robot_classes.argtypes = [vp, C.c_int, C.POINTER(RobotClass), vp]
     lib.rda_set_robot_class_index.argtypes = [vp, vp, vp]
+    lib.rda_set_obstacle_ids.argtypes = [vp, vp, vp]
     lib.rda_reset.argtypes = [vp, vp]
     lib.rda_cold_start.argtypes = [vp, vp]
     lib.rda_solve.argtypes = [vp, C.POINTER(Inputs), C.POINTER(Outputs), C.c_int, C.c_float, vp]
@@ -121,6 +123,9 @@ def load():
     lib.rda_fleet_plan_shapes.argtypes = [i, i, i, f, f, i, i, vp, f] + [vp] * 13
     lib.rda_convert_fleet_plan_obstacles.argtypes = [i, i, i, i, i, f, i, i] + [vp] * 21
     lib.rda_convert_world_obstacles_horizon.argtypes = [i, i, i, i, i, f, i, vp, vp, i, i, vp, f] + [vp] * 22
+    lib.rda_convert_obstacles_ids.argtypes = [i, i, i, i, i, f, i, i] + [vp] * 13
+    lib.rda_convert_world_obstacles_ids.argtypes = [i, i, i, i, i, f, i, i] + [vp] * 22
+    lib.rda_convert_world_obstacles_horizon_ids.argtypes = [i, i, i, i, i, f, i, vp, vp, i, i, vp, f] + [vp] * 23
     for name in EXPORTS:
         if name != 'rda_version':
             getattr(lib, name).restype = C.c_int

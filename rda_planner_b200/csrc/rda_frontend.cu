@@ -50,12 +50,14 @@ __global__ void k_pre_process_paths(int B, int T, int dynamics, float dt, float 
   if (solver_speed) solver_speed[b] = ref_speed[b] * (float)gear;
 }
 
-// one CTA per instance: keys -> stable ranks -> rows of the N slots
-__global__ void __launch_bounds__(RDA_MAX_SHAPES)
-k_convert_obstacles(int B, int M, int N, int T, int E, float dt, int time_varying, int order, const float* state,
-                    const int* shape_kind, const int* shape_nv, const float* shape_xy, const float* shape_radius,
-                    const float* shape_vel, const int* shape_count, float* obs_A, float* obs_b, int* obs_kind,
-                    int* obs_count) {
+// one CTA per instance: keys -> stable ranks -> rows of the N slots.  kIds: also the list position of each slot's
+// shape into obs_id [B][N] (-1 for an empty list).
+template <bool kIds>
+__device__ __forceinline__ void convert_obstacles(int B, int M, int N, int T, int E, float dt, int time_varying, int order,
+                                                  const float* state, const int* shape_kind, const int* shape_nv,
+                                                  const float* shape_xy, const float* shape_radius, const float* shape_vel,
+                                                  const int* shape_count, float* obs_A, float* obs_b, int* obs_kind,
+                                                  int* obs_count, int* obs_id) {
   __shared__ double keys[RDA_MAX_SHAPES];
   __shared__ int sorted[RDA_MAX_SHAPES];
   const int b = blockIdx.x;
@@ -84,9 +86,11 @@ k_convert_obstacles(int B, int M, int N, int T, int E, float dt, int time_varyin
     if (count == 0) {
       for (int i = 0; i < Tc * E; ++i) { A[2 * i] = 0.f; A[2 * i + 1] = 0.f; bb[i] = 0.f; }
       obs_kind[(size_t)b * N + n] = RDA_OBS_POLYGON;
+      if (kIds) obs_id[(size_t)b * N + n] = -1;
       continue;
     }
     const int src = sorted[n < count ? n : count - 1];
+    if (kIds) obs_id[(size_t)b * N + n] = src;
     const int kind = shape_kind[sb + src], nv = shape_nv[sb + src];
     const float* xy = shape_xy + (sb + src) * RDA_MAX_EDGE * 2;
     const double rad = shape_radius[sb + src];
@@ -94,6 +98,24 @@ k_convert_obstacles(int B, int M, int N, int T, int E, float dt, int time_varyin
     obs_kind[(size_t)b * N + n] = kind;
     for (int t = 0; t < Tc; ++t) obstacle_rows(kind, nv, xy, rad, vx, vy, t, (double)dt, E, A + (size_t)t * E * 2, bb + (size_t)t * E);
   }
+}
+
+__global__ void __launch_bounds__(RDA_MAX_SHAPES)
+k_convert_obstacles(int B, int M, int N, int T, int E, float dt, int time_varying, int order, const float* state,
+                    const int* shape_kind, const int* shape_nv, const float* shape_xy, const float* shape_radius,
+                    const float* shape_vel, const int* shape_count, float* obs_A, float* obs_b, int* obs_kind,
+                    int* obs_count) {
+  convert_obstacles<false>(B, M, N, T, E, dt, time_varying, order, state, shape_kind, shape_nv, shape_xy, shape_radius,
+                           shape_vel, shape_count, obs_A, obs_b, obs_kind, obs_count, nullptr);
+}
+
+__global__ void __launch_bounds__(RDA_MAX_SHAPES)
+k_convert_obstacles_ids(int B, int M, int N, int T, int E, float dt, int time_varying, int order, const float* state,
+                        const int* shape_kind, const int* shape_nv, const float* shape_xy, const float* shape_radius,
+                        const float* shape_vel, const int* shape_count, float* obs_A, float* obs_b, int* obs_kind,
+                        int* obs_count, int* obs_id) {
+  convert_obstacles<true>(B, M, N, T, E, dt, time_varying, order, state, shape_kind, shape_nv, shape_xy, shape_radius,
+                          shape_vel, shape_count, obs_A, obs_b, obs_kind, obs_count, obs_id);
 }
 
 // Shared worlds: one CTA per robot scans its world in tiles of kWorldTile shapes, one key per thread, and keeps the
@@ -199,16 +221,35 @@ __device__ __forceinline__ void world_slots(int tid, int b, int B, int N, int T,
   }
 }
 
+// The obstacle id of each of the N slots world_slots writes for robot b, into obs_id [B][N]: the flat shape index of a
+// world shape, mate_base + m for map-mate robot m, -1 for an empty list.
+__device__ __forceinline__ void world_slot_ids(int tid, int b, int B, int N, int count, const ShapeList& L,
+                                               const int* kept_idx, const int* fleet_robot, int mate_base, int* obs_id) {
+  for (int n = tid; n < N; n += kWorldTile) {
+    int id = -1;
+    if (count > 0) {
+      int src = kept_idx ? kept_idx[n < count ? n : count - 1] : (n < count ? n : count - 1);
+      if (src < 0 || src >= count) src = count - 1;
+      bool mate;
+      const size_t s = list_entry(L, src, fleet_robot, b, B, &mate);
+      id = mate ? mate_base + (int)s : (int)s;
+    }
+    obs_id[(size_t)b * N + n] = id;
+  }
+}
+
 // kPlan: map-mates are read along their plans, fleet_plan_xy [B][T+1][RDA_MAX_EDGE][2] (time-varying output only);
 // the variant without plans never reads it, and compiles to the code it had before plans existed.
-template <bool kPlan>
-__global__ void __launch_bounds__(kWorldTile)
-k_convert_world_obstacles(int B, int W, int N, int T, int E, float dt, int time_varying, int order, const float* state,
-                          const int* world_start, const int* robot_world, const int* shape_kind, const int* shape_nv,
-                          const float* shape_xy, const float* shape_radius, const float* shape_vel,
-                          const int* fleet_start, const int* fleet_robot, const int* fleet_kind, const int* fleet_nv,
-                          const float* fleet_xy, const float* fleet_radius, const float* fleet_vel,
-                          const float* fleet_plan_xy, float* obs_A, float* obs_b, int* obs_kind, int* obs_count) {
+// kIds: also the slots' obstacle ids (world_slots) into obs_id.
+template <bool kPlan, bool kIds>
+__device__ __forceinline__ void convert_world(int B, int W, int N, int T, int E, float dt, int time_varying, int order,
+                                              const float* state, const int* world_start, const int* robot_world,
+                                              const int* shape_kind, const int* shape_nv, const float* shape_xy,
+                                              const float* shape_radius, const float* shape_vel, const int* fleet_start,
+                                              const int* fleet_robot, const int* fleet_kind, const int* fleet_nv,
+                                              const float* fleet_xy, const float* fleet_radius, const float* fleet_vel,
+                                              const float* fleet_plan_xy, float* obs_A, float* obs_b, int* obs_kind,
+                                              int* obs_count, int* obs_id) {
   // dynamic shared memory (order != 0): kept keys [2][N], candidate keys [2][tile], kept indices [2][N],
   // candidate indices [2][tile]; the kept list is double-buffered, candidates are gathered then sorted
   extern __shared__ double sh[];
@@ -268,6 +309,30 @@ k_convert_world_obstacles(int B, int W, int N, int T, int E, float dt, int time_
   world_slots<kPlan>(tid, b, B, N, T, E, dt, time_varying, count, L, kept_idx, shape_kind, shape_nv, shape_xy,
                      shape_radius, shape_vel, fleet_robot, fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel,
                      fleet_plan_xy, obs_A, obs_b, obs_kind);
+  if (kIds) world_slot_ids(tid, b, B, N, count, L, kept_idx, fleet_robot, world_start[W], obs_id);
+}
+
+// The parameter lists of the world kernels and the arguments that forward them.  The launchers
+// (launch_world_obstacles, launch_world_obstacles_horizon) name their parameters alike and forward them with the same
+// macros; all four are undefined after the launchers.
+#define RDA_WORLD_PARAMS                                                                                               \
+  int B, int W, int N, int T, int E, float dt, int time_varying, int order, const float *state, const int *world_start, \
+      const int *robot_world, const int *shape_kind, const int *shape_nv, const float *shape_xy,                       \
+      const float *shape_radius, const float *shape_vel, const int *fleet_start, const int *fleet_robot,                 \
+      const int *fleet_kind, const int *fleet_nv, const float *fleet_xy, const float *fleet_radius,                      \
+      const float *fleet_vel, const float *fleet_plan_xy, float *obs_A, float *obs_b, int *obs_kind, int *obs_count
+#define RDA_WORLD_ARGS                                                                                                 \
+  B, W, N, T, E, dt, time_varying, order, state, world_start, robot_world, shape_kind, shape_nv, shape_xy, shape_radius, \
+      shape_vel, fleet_start, fleet_robot, fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel, fleet_plan_xy,      \
+      obs_A, obs_b, obs_kind, obs_count
+
+template <bool kPlan>
+__global__ void __launch_bounds__(kWorldTile) k_convert_world_obstacles(RDA_WORLD_PARAMS) {
+  convert_world<kPlan, false>(RDA_WORLD_ARGS, nullptr);
+}
+template <bool kPlan>
+__global__ void __launch_bounds__(kWorldTile) k_convert_world_obstacles_ids(RDA_WORLD_PARAMS, int* obs_id) {
+  convert_world<kPlan, true>(RDA_WORLD_ARGS, obs_id);
 }
 
 // Horizon order (rda_convert_world_obstacles_horizon): the tiles, candidates and merge of k_convert_world_obstacles
@@ -282,17 +347,21 @@ k_convert_world_obstacles(int B, int W, int N, int T, int E, float dt, int time_
 // The selection is therefore that of sorting every exact key.  EC / RC: compile-time caps of the obstacle rows and
 // body vertices (plan_clearance_cell).  The body (the one body, or body_xy_b [b] / body_radius_b [b]) and the horizon
 // disc are staged once in shared memory.
-template <int EC, int RC, bool kPlan>
-__global__ void __launch_bounds__(kWorldTile)
-k_convert_world_obstacles_horizon(int B, int W, int N, int T, int E, float dt, int time_varying, const float* nom_s,
-                                  const float* ref_s, int body_kind, int body_nv, const float* body_xy,
-                                  float body_radius, const float* body_xy_b, const float* body_radius_b,
-                                  const int* world_start, const int* robot_world, const int* shape_kind,
-                                  const int* shape_nv, const float* shape_xy, const float* shape_radius,
-                                  const float* shape_vel, const int* fleet_start, const int* fleet_robot,
-                                  const int* fleet_kind, const int* fleet_nv, const float* fleet_xy,
-                                  const float* fleet_radius, const float* fleet_vel, const float* fleet_plan_xy,
-                                  float* obs_A, float* obs_b, int* obs_kind, int* obs_count) {
+#define RDA_HORIZON_PARAMS                                                                                             \
+  int B, int W, int N, int T, int E, float dt, int time_varying, const float *nom_s, const float *ref_s, int body_kind, \
+      int body_nv, const float *body_xy, float body_radius, const float *body_xy_b, const float *body_radius_b,        \
+      const int *world_start, const int *robot_world, const int *shape_kind, const int *shape_nv,                      \
+      const float *shape_xy, const float *shape_radius, const float *shape_vel, const int *fleet_start,                \
+      const int *fleet_robot, const int *fleet_kind, const int *fleet_nv, const float *fleet_xy,                       \
+      const float *fleet_radius, const float *fleet_vel, const float *fleet_plan_xy, float *obs_A, float *obs_b,        \
+      int *obs_kind, int *obs_count
+#define RDA_HORIZON_ARGS                                                                                               \
+  B, W, N, T, E, dt, time_varying, nom_s, ref_s, body_kind, body_nv, body_xy, body_radius, body_xy_b, body_radius_b,     \
+      world_start, robot_world, shape_kind, shape_nv, shape_xy, shape_radius, shape_vel, fleet_start, fleet_robot,      \
+      fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel, fleet_plan_xy, obs_A, obs_b, obs_kind, obs_count
+
+template <int EC, int RC, bool kPlan, bool kIds>
+__device__ __forceinline__ void convert_world_horizon(RDA_HORIZON_PARAMS, int* obs_id) {
   // dynamic shared memory: as k_convert_world_obstacles, then the survivors of a tile [tile]
   extern __shared__ double sh[];
   __shared__ int n_surv, n_cand;
@@ -393,6 +462,16 @@ k_convert_world_obstacles_horizon(int B, int W, int N, int T, int E, float dt, i
   world_slots<kPlan>(tid, b, B, N, T, E, dt, time_varying, count, L, kept_idx, shape_kind, shape_nv, shape_xy,
                      shape_radius, shape_vel, fleet_robot, fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel,
                      fleet_plan_xy, obs_A, obs_b, obs_kind);
+  if (kIds) world_slot_ids(tid, b, B, N, count, L, kept_idx, fleet_robot, world_start[W], obs_id);
+}
+
+template <int EC, int RC, bool kPlan>
+__global__ void __launch_bounds__(kWorldTile) k_convert_world_obstacles_horizon(RDA_HORIZON_PARAMS) {
+  convert_world_horizon<EC, RC, kPlan, false>(RDA_HORIZON_ARGS, nullptr);
+}
+template <int EC, int RC, bool kPlan>
+__global__ void __launch_bounds__(kWorldTile) k_convert_world_obstacles_horizon_ids(RDA_HORIZON_PARAMS, int* obs_id) {
+  convert_world_horizon<EC, RC, kPlan, true>(RDA_HORIZON_ARGS, obs_id);
 }
 
 // Each robot of a fleet as a raw shape for its map-mates (fleet_shape), one thread per robot: its body at its pose,
@@ -473,7 +552,7 @@ int launch_world_obstacles(bool fleet, int B, int W, int N, int T, int E, float 
                            const int32_t* fleet_robot, const int32_t* fleet_kind, const int32_t* fleet_nv,
                            const float* fleet_xy, const float* fleet_radius, const float* fleet_vel,
                            const float* fleet_plan_xy, float* obs_A, float* obs_b, int32_t* obs_kind,
-                           int32_t* obs_count, cudaStream_t stream) {
+                           int32_t* obs_count, int32_t* obs_id, cudaStream_t stream) {
   if (B < 1 || W < 1 || N < 1 || T < 1) return RDA_E_ARG;
   if (N > RDA_MAX_WORLD_SLOTS || E < 3 || E > RDA_MAX_EDGE) return RDA_E_UNSUPPORTED;
   if (!world_start || !shape_kind || !shape_nv || !shape_xy || !shape_radius || !shape_vel) return RDA_E_ARG;
@@ -482,10 +561,12 @@ int launch_world_obstacles(bool fleet, int B, int W, int N, int T, int E, float 
     return RDA_E_ARG;
   if (fleet_plan_xy && (!fleet || !time_varying)) return RDA_E_ARG;
   const size_t smem = order ? (size_t)(2 * N + 2 * kWorldTile) * (sizeof(double) + sizeof(int)) : 0;
-  (fleet_plan_xy ? k_convert_world_obstacles<true> : k_convert_world_obstacles<false>)<<<B, kWorldTile, smem, stream>>>(
-      B, W, N, T, E, dt, time_varying, order, state, world_start, robot_world, shape_kind, shape_nv, shape_xy,
-      shape_radius, shape_vel, fleet_start, fleet_robot, fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel,
-      fleet_plan_xy, obs_A, obs_b, obs_kind, obs_count);
+  if (obs_id)
+    (fleet_plan_xy ? k_convert_world_obstacles_ids<true> : k_convert_world_obstacles_ids<false>)<<<B, kWorldTile, smem, stream>>>(
+        RDA_WORLD_ARGS, obs_id);
+  else
+    (fleet_plan_xy ? k_convert_world_obstacles<true> : k_convert_world_obstacles<false>)<<<B, kWorldTile, smem, stream>>>(
+        RDA_WORLD_ARGS);
   RDA_CUDA(cudaGetLastError());
   return 0;
 }
@@ -501,7 +582,7 @@ int launch_world_obstacles_horizon(int B, int W, int N, int T, int E, float dt, 
                                    const int32_t* fleet_kind, const int32_t* fleet_nv, const float* fleet_xy,
                                    const float* fleet_radius, const float* fleet_vel, const float* fleet_plan_xy,
                                    float* obs_A, float* obs_b, int32_t* obs_kind, int32_t* obs_count,
-                                   cudaStream_t stream) {
+                                   int32_t* obs_id, cudaStream_t stream) {
   if (B < 1 || W < 1 || N < 1 || T < 1) return RDA_E_ARG;
   if (N > RDA_MAX_WORLD_SLOTS || E < 3 || E > RDA_MAX_EDGE) return RDA_E_UNSUPPORTED;
   if (body_kind == RDA_OBS_POLYGON) {
@@ -517,17 +598,24 @@ int launch_world_obstacles_horizon(int B, int W, int N, int T, int E, float dt, 
   if (fleet_plan_xy && (!fleet || !time_varying)) return RDA_E_ARG;
   const bool small = E <= 4 && (body_kind == RDA_OBS_CIRCLE || body_nv <= 4);
   const bool plan = fleet_plan_xy != nullptr;
-  auto k = small ? (plan ? k_convert_world_obstacles_horizon<4, 4, true> : k_convert_world_obstacles_horizon<4, 4, false>)
-                 : (plan ? k_convert_world_obstacles_horizon<8, 8, true> : k_convert_world_obstacles_horizon<8, 8, false>);
   const size_t smem = (size_t)(2 * N + 2 * kWorldTile) * (sizeof(double) + sizeof(int)) + kWorldTile * sizeof(int);
-  k<<<B, kWorldTile, smem, stream>>>(B, W, N, T, E, dt, time_varying, nom_s, ref_s, body_kind, body_nv, body_xy,
-                                     body_radius, body_xy_b, body_radius_b, world_start, robot_world, shape_kind,
-                                     shape_nv, shape_xy, shape_radius, shape_vel, fleet_start, fleet_robot, fleet_kind,
-                                     fleet_nv, fleet_xy, fleet_radius, fleet_vel, fleet_plan_xy, obs_A, obs_b, obs_kind,
-                                     obs_count);
+  if (obs_id) {
+    auto k = small ? (plan ? k_convert_world_obstacles_horizon_ids<4, 4, true> : k_convert_world_obstacles_horizon_ids<4, 4, false>)
+                   : (plan ? k_convert_world_obstacles_horizon_ids<8, 8, true> : k_convert_world_obstacles_horizon_ids<8, 8, false>);
+    k<<<B, kWorldTile, smem, stream>>>(RDA_HORIZON_ARGS, obs_id);
+  } else {
+    auto k = small ? (plan ? k_convert_world_obstacles_horizon<4, 4, true> : k_convert_world_obstacles_horizon<4, 4, false>)
+                   : (plan ? k_convert_world_obstacles_horizon<8, 8, true> : k_convert_world_obstacles_horizon<8, 8, false>);
+    k<<<B, kWorldTile, smem, stream>>>(RDA_HORIZON_ARGS);
+  }
   RDA_CUDA(cudaGetLastError());
   return 0;
 }
+
+#undef RDA_WORLD_PARAMS
+#undef RDA_WORLD_ARGS
+#undef RDA_HORIZON_PARAMS
+#undef RDA_HORIZON_ARGS
 
 }  // namespace
 
@@ -634,7 +722,7 @@ int rda_convert_world_obstacles(int B, int W, int N, int T, int E, float dt, int
   return launch_world_obstacles(false, B, W, N, T, E, dt, time_varying, order, state, world_start, robot_world,
                                 shape_kind, shape_nv, shape_xy, shape_radius, shape_vel, nullptr, nullptr, nullptr,
                                 nullptr, nullptr, nullptr, nullptr, nullptr, obs_A, obs_b, obs_kind, obs_count,
-                                (cudaStream_t)stream);
+                                nullptr, (cudaStream_t)stream);
 }
 
 int rda_fleet_shapes(int B, int T, int dynamics, int body_kind, int body_nv, const float* body_xy, float body_radius,
@@ -686,7 +774,7 @@ int rda_convert_fleet_obstacles(int B, int W, int N, int T, int E, float dt, int
   return launch_world_obstacles(true, B, W, N, T, E, dt, time_varying, order, state, world_start, robot_world,
                                 shape_kind, shape_nv, shape_xy, shape_radius, shape_vel, fleet_start, fleet_robot,
                                 fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel, nullptr, obs_A, obs_b,
-                                obs_kind, obs_count, (cudaStream_t)stream);
+                                obs_kind, obs_count, nullptr, (cudaStream_t)stream);
 }
 
 int rda_fleet_plan_shapes(int B, int T, int dynamics, float dt, float wheelbase, int body_kind, int body_nv,
@@ -722,7 +810,7 @@ int rda_convert_fleet_plan_obstacles(int B, int W, int N, int T, int E, float dt
   return launch_world_obstacles(true, B, W, N, T, E, dt, time_varying, order, state, world_start, robot_world,
                                 shape_kind, shape_nv, shape_xy, shape_radius, shape_vel, fleet_start, fleet_robot,
                                 fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel, fleet_plan_xy, obs_A, obs_b,
-                                obs_kind, obs_count, (cudaStream_t)stream);
+                                obs_kind, obs_count, nullptr, (cudaStream_t)stream);
 }
 
 int rda_convert_world_obstacles_horizon(int B, int W, int N, int T, int E, float dt, int time_varying,
@@ -740,7 +828,59 @@ int rda_convert_world_obstacles_horizon(int B, int W, int N, int T, int E, float
                                         body_radius, body_xy_b, body_radius_b, world_start, robot_world, shape_kind,
                                         shape_nv, shape_xy, shape_radius, shape_vel, fleet_start, fleet_robot,
                                         fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel, fleet_plan_xy, obs_A,
-                                        obs_b, obs_kind, obs_count, (cudaStream_t)stream);
+                                        obs_b, obs_kind, obs_count, nullptr, (cudaStream_t)stream);
+}
+
+int rda_convert_obstacles_ids(int B, int M, int N, int T, int E, float dt, int time_varying, int order,
+                              const float* state, const int32_t* shape_kind, const int32_t* shape_nv,
+                              const float* shape_xy, const float* shape_radius, const float* shape_vel,
+                              const int32_t* shape_count, float* obs_A, float* obs_b, int32_t* obs_kind,
+                              int32_t* obs_count, int32_t* obs_id, void* stream) {
+  if (B < 1 || N < 1 || T < 1 || M < 1) return RDA_E_ARG;
+  if (M > RDA_MAX_SHAPES || E < 3 || E > RDA_MAX_EDGE) return RDA_E_UNSUPPORTED;
+  if (!shape_kind || !shape_nv || !shape_xy || !shape_radius || !shape_vel || !shape_count) return RDA_E_ARG;
+  if (!obs_A || !obs_b || !obs_kind || !obs_count || !obs_id || (order && !state)) return RDA_E_ARG;
+  k_convert_obstacles_ids<<<B, RDA_MAX_SHAPES, 0, (cudaStream_t)stream>>>(B, M, N, T, E, dt, time_varying, order, state,
+                                                                         shape_kind, shape_nv, shape_xy, shape_radius,
+                                                                         shape_vel, shape_count, obs_A, obs_b, obs_kind,
+                                                                         obs_count, obs_id);
+  RDA_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int rda_convert_world_obstacles_ids(int B, int W, int N, int T, int E, float dt, int time_varying, int order,
+                                    const float* state, const int32_t* world_start, const int32_t* robot_world,
+                                    const int32_t* shape_kind, const int32_t* shape_nv, const float* shape_xy,
+                                    const float* shape_radius, const float* shape_vel, const int32_t* fleet_start,
+                                    const int32_t* fleet_robot, const int32_t* fleet_kind, const int32_t* fleet_nv,
+                                    const float* fleet_xy, const float* fleet_radius, const float* fleet_vel,
+                                    const float* fleet_plan_xy, float* obs_A, float* obs_b, int32_t* obs_kind,
+                                    int32_t* obs_count, int32_t* obs_id, void* stream) {
+  if (!obs_id) return RDA_E_ARG;
+  return launch_world_obstacles(fleet_start != nullptr, B, W, N, T, E, dt, time_varying, order, state, world_start,
+                                robot_world, shape_kind, shape_nv, shape_xy, shape_radius, shape_vel, fleet_start,
+                                fleet_robot, fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel, fleet_plan_xy,
+                                obs_A, obs_b, obs_kind, obs_count, obs_id, (cudaStream_t)stream);
+}
+
+int rda_convert_world_obstacles_horizon_ids(int B, int W, int N, int T, int E, float dt, int time_varying,
+                                            const float* nom_s, const float* ref_s, int body_kind, int body_nv,
+                                            const float* body_xy, float body_radius, const float* body_xy_b,
+                                            const float* body_radius_b, const int32_t* world_start,
+                                            const int32_t* robot_world, const int32_t* shape_kind,
+                                            const int32_t* shape_nv, const float* shape_xy, const float* shape_radius,
+                                            const float* shape_vel, const int32_t* fleet_start,
+                                            const int32_t* fleet_robot, const int32_t* fleet_kind,
+                                            const int32_t* fleet_nv, const float* fleet_xy, const float* fleet_radius,
+                                            const float* fleet_vel, const float* fleet_plan_xy, float* obs_A,
+                                            float* obs_b, int32_t* obs_kind, int32_t* obs_count, int32_t* obs_id,
+                                            void* stream) {
+  if (!obs_id) return RDA_E_ARG;
+  return launch_world_obstacles_horizon(B, W, N, T, E, dt, time_varying, nom_s, ref_s, body_kind, body_nv, body_xy,
+                                        body_radius, body_xy_b, body_radius_b, world_start, robot_world, shape_kind,
+                                        shape_nv, shape_xy, shape_radius, shape_vel, fleet_start, fleet_robot,
+                                        fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel, fleet_plan_xy, obs_A,
+                                        obs_b, obs_kind, obs_count, obs_id, (cudaStream_t)stream);
 }
 
 int rda_post_process(int B, int T, int P, int goal_index_threshold, const int32_t* near_index, float* u_opt,

@@ -19,6 +19,7 @@
 #include "cell_lean2.cuh"
 #include "cell_disc_robot.cuh"
 #include "plan_clearance.cuh"
+#include "obstacle_ids.cuh"
 
 using namespace rda;
 
@@ -92,6 +93,10 @@ struct rda_handle {
   int ncls;
   int* cls_idx;
   int cls_on;
+  // the obstacle id of every slot in the last solve [B][N] (rda_set_obstacle_ids; allocated on the first call), held
+  // while ids_on is set
+  int* obs_id;
+  int ids_on;
 };
 
 #define RDA_CUDA(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) return (int)e_; } while (0)
@@ -1240,6 +1245,68 @@ __global__ void k_fill(float* p, float v, size_t n) {
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) p[i] = v;
 }
 
+// rda_set_obstacle_ids: one CTA per instance moves the per-slot warm start to the slots its obstacles went to.  The
+// match (obstacle_ids.cuh) is one thread per slot on the ids in shared memory; an instance whose slots all keep their
+// state stops there.  Otherwise the CTA copies the instance's per-slot planes into its own regions of the record lists,
+// which the cell passes refill from scratch in every iteration (lam, mu: rec_a; z, zeta, xi, coef and feat: rec_b),
+// then writes each moved slot from its source slot, or the cold-start zeros.  ids [B][N] (the handle's) receives cur.
+constexpr int REMAP_THREADS = 256;
+__global__ void __launch_bounds__(REMAP_THREADS) k_remap_slots(DevPtrs d, int* __restrict__ ids,
+                                                               const int* __restrict__ cur_ids) {
+  extern __shared__ int remap_sh[];                    // prev [N], cur [N], src [N]
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int N = d.N, T = d.T, E = d.E, R = d.R, NT = N * T;
+  int* prev = remap_sh;
+  int* cur = prev + N;
+  int* src = cur + N;
+  int* idb = ids + (size_t)b * N;
+  for (int n = tid; n < N; n += REMAP_THREADS) { prev[n] = idb[n]; cur[n] = cur_ids[(size_t)b * N + n]; }
+  __syncthreads();
+  int moved = 0;
+  for (int n = tid; n < N; n += REMAP_THREADS) {
+    const int s = obstacle_slot_source(prev, cur, N, n);
+    src[n] = s;
+    moved |= s != n;
+    idb[n] = cur[n];
+  }
+  if (!__syncthreads_or(moved)) return;
+  float* lam = d.lam + (size_t)b * N * E * T;
+  float* mu = d.mu + (size_t)b * N * R * T;
+  // the nine [N][T] planes of the instance: z, zeta, xi (2), coef (5)
+  auto plane = [&](int p) -> float* {
+    return p == 0 ? d.z + (size_t)b * NT : p == 1 ? d.zeta + (size_t)b * NT
+         : p < 4 ? d.xi + ((size_t)b * 2 + (p - 2)) * NT : d.coef + ((size_t)b * 5 + (p - 4)) * NT;
+  };
+  unsigned char* feat = d.feat ? d.feat + (size_t)b * NT : nullptr;
+  float* sa = (float*)(d.rec_a + (size_t)b * NT);     // 20 floats per cell: lam, mu (E + R <= 16)
+  float* sb = (float*)(d.rec_b + (size_t)b * NT);     // the nine planes, then feat (9 floats + 1 byte <= 20 floats)
+  unsigned char* sf = (unsigned char*)(sb + 9 * NT);
+  const int NET = N * E * T, NRT = N * R * T;
+  for (int i = tid; i < NET; i += REMAP_THREADS) sa[i] = lam[i];
+  for (int i = tid; i < NRT; i += REMAP_THREADS) sa[NET + i] = mu[i];
+  for (int i = tid; i < 9 * NT; i += REMAP_THREADS) sb[i] = plane(i / NT)[i % NT];
+  if (feat)
+    for (int i = tid; i < NT; i += REMAP_THREADS) sf[i] = feat[i];
+  __syncthreads();
+  for (int i = tid; i < NET; i += REMAP_THREADS) {
+    const int n = i / (E * T), s = src[n];
+    if (s != n) lam[i] = s < 0 ? 0.f : sa[i + (s - n) * E * T];
+  }
+  for (int i = tid; i < NRT; i += REMAP_THREADS) {
+    const int n = i / (R * T), s = src[n];
+    if (s != n) mu[i] = s < 0 ? 0.f : sa[NET + i + (s - n) * R * T];
+  }
+  for (int i = tid; i < 9 * NT; i += REMAP_THREADS) {
+    const int r = i % NT, n = r / T, s = src[n];
+    if (s != n) plane(i / NT)[r] = s < 0 ? 0.f : sb[i + (s - n) * T];
+  }
+  if (feat)
+    for (int i = tid; i < NT; i += REMAP_THREADS) {
+      const int n = i / T, s = src[n];
+      if (s != n) feat[i] = s < 0 ? (unsigned char)0 : sf[i + (s - n) * T];
+    }
+}
+
 // (value, index) of two candidates: the smaller value, the smaller index among equal values (any reduction order gives
 // the same result)
 __device__ __forceinline__ void clear_min(float& v, int& i, float ov, int oi) {
@@ -1467,6 +1534,7 @@ int rda_destroy(rda_handle* h) {
   if (h->cls_ra) cudaFree(h->cls_ra);
   if (h->cls_kin) cudaFree(h->cls_kin);
   if (h->cls_idx) cudaFree(h->cls_idx);
+  if (h->obs_id) cudaFree(h->obs_id);
   if (h->ev_fork) cudaEventDestroy(h->ev_fork);
   for (int p = 0; p < 3; ++p) {
     if (h->ev_join[p]) cudaEventDestroy(h->ev_join[p]);
@@ -1540,6 +1608,24 @@ int rda_set_robot_class_index(rda_handle* h, const int32_t* robot_class, void* s
   RDA_CUDA(cudaMemcpyAsync(h->cls_idx, robot_class, (size_t)h->B * sizeof(int), cudaMemcpyDeviceToDevice,
                            (cudaStream_t)stream));
   h->cls_on = 1;
+  return 0;
+}
+
+int rda_set_obstacle_ids(rda_handle* h, const int32_t* obs_id, void* stream) {
+  if (!h) return RDA_E_ARG;
+  if (!obs_id) { h->ids_on = 0; return 0; }             // the storage stays for the next ids
+  const size_t smem = (size_t)h->N * 3 * sizeof(int);
+  if (smem > 48 * 1024) return RDA_E_UNSUPPORTED;
+  const size_t n = (size_t)h->B * h->N;
+  if (!h->obs_id) RDA_CUDA(cudaMalloc((void**)&h->obs_id, (n ? n : 1) * sizeof(int)));
+  cudaStream_t s = (cudaStream_t)stream;
+  if (!h->ids_on || h->N == 0) {
+    RDA_CUDA(cudaMemcpyAsync(h->obs_id, obs_id, n * sizeof(int), cudaMemcpyDeviceToDevice, s));
+    h->ids_on = 1;
+    return 0;
+  }
+  k_remap_slots<<<h->B, REMAP_THREADS, smem, s>>>(dev_ptrs(h), h->obs_id, obs_id);
+  RDA_CUDA(cudaGetLastError());
   return 0;
 }
 

@@ -172,9 +172,11 @@ def pre_process_batch(state, cur_vel, ref_speed, path, start_index, dynamics, dt
     return nom, ref, near
 
 
-def convert_obstacles_batch(shapes, state, N, T, E, dt, time_varying=False, order=True):
+def convert_obstacles_batch(shapes, state, N, T, E, dt, time_varying=False, order=True, ids=False):
     """shapes: dict of CUDA tensors (kind, nv [B,M] int32; xy [B,M,8,2]; radius [B,M]; vel [B,M,2];
-    count [B] int32).  Returns obs_A [B,N,Tc,E,2], obs_b [B,N,Tc,E], obs_kind [B,N], obs_count [B]."""
+    count [B] int32).  Returns obs_A [B,N,Tc,E,2], obs_b [B,N,Tc,E], obs_kind [B,N], obs_count [B], and with ids also
+    obs_id [B,N] int32: the position of each slot's shape in the robot's list (-1 for an empty list), for
+    RDA_solver.set_obstacle_ids."""
     lib = _cabi.load()
     dev = shapes['kind'].device
     B, M = shapes['kind'].shape
@@ -183,20 +185,25 @@ def convert_obstacles_batch(shapes, state, N, T, E, dt, time_varying=False, orde
     b = torch.empty((B, N, Tc, E), dtype=torch.float32, device=dev)
     kind = torch.empty((B, N), dtype=torch.int32, device=dev)
     count = torch.empty(B, dtype=torch.int32, device=dev)
+    args = (B, M, N, T, E, dt, int(time_varying), int(order), _ptr(state), _ptr(shapes['kind']), _ptr(shapes['nv']),
+            _ptr(shapes['xy']), _ptr(shapes['radius']), _ptr(shapes['vel']), _ptr(shapes['count']), _ptr(A), _ptr(b),
+            _ptr(kind), _ptr(count))
     with torch.cuda.device(dev):
-        _cabi.check(lib.rda_convert_obstacles(B, M, N, T, E, dt, int(time_varying), int(order), _ptr(state),
-                                              _ptr(shapes['kind']), _ptr(shapes['nv']), _ptr(shapes['xy']),
-                                              _ptr(shapes['radius']), _ptr(shapes['vel']), _ptr(shapes['count']),
-                                              _ptr(A), _ptr(b), _ptr(kind), _ptr(count), _stream(dev)),
-                    'rda_convert_obstacles')
+        if ids:
+            obs_id = torch.empty((B, N), dtype=torch.int32, device=dev)
+            _cabi.check(lib.rda_convert_obstacles_ids(*args, _ptr(obs_id), _stream(dev)), 'rda_convert_obstacles_ids')
+            return A, b, kind, count, obs_id
+        _cabi.check(lib.rda_convert_obstacles(*args, _stream(dev)), 'rda_convert_obstacles')
     return A, b, kind, count
 
 
-def convert_world_obstacles_batch(world, state, robot_world, N, T, E, dt, time_varying=False, order=True):
+def convert_world_obstacles_batch(world, state, robot_world, N, T, E, dt, time_varying=False, order=True, ids=False):
     """world: dict of CUDA tensors from pack_worlds (kind, nv [S] int32; xy [S,8,2]; radius [S]; vel [S,2];
     start [W+1] int32); robot_world [B] int32 or None (every robot in world 0).  Each robot gets the N nearest
     shapes of its world (order) or its first N, as convert_obstacles_batch would given the whole world as its
-    list.  Returns obs_A [B,N,Tc,E,2], obs_b [B,N,Tc,E], obs_kind [B,N], obs_count [B] (the world sizes)."""
+    list.  Returns obs_A [B,N,Tc,E,2], obs_b [B,N,Tc,E], obs_kind [B,N], obs_count [B] (the world sizes), and with ids
+    also obs_id [B,N] int32: the flat index of each slot's shape in the packed worlds (-1 for an empty world), for
+    RDA_solver.set_obstacle_ids."""
     lib = _cabi.load()
     dev = state.device
     B, W = state.shape[0], world['start'].shape[0] - 1
@@ -205,6 +212,15 @@ def convert_world_obstacles_batch(world, state, robot_world, N, T, E, dt, time_v
     b = torch.empty((B, N, Tc, E), dtype=torch.float32, device=dev)
     kind = torch.empty((B, N), dtype=torch.int32, device=dev)
     count = torch.empty(B, dtype=torch.int32, device=dev)
+    if ids:
+        obs_id = torch.empty((B, N), dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            _cabi.check(lib.rda_convert_world_obstacles_ids(
+                B, W, N, T, E, dt, int(time_varying), int(order), _ptr(state), _ptr(world['start']), _ptr(robot_world),
+                _ptr(world['kind']), _ptr(world['nv']), _ptr(world['xy']), _ptr(world['radius']), _ptr(world['vel']),
+                *(None,) * 8, _ptr(A), _ptr(b), _ptr(kind), _ptr(count), _ptr(obs_id), _stream(dev)),
+                'rda_convert_world_obstacles_ids')
+        return A, b, kind, count, obs_id
     with torch.cuda.device(dev):
         _cabi.check(lib.rda_convert_world_obstacles(B, W, N, T, E, dt, int(time_varying), int(order), _ptr(state),
                                                     _ptr(world['start']), _ptr(robot_world), _ptr(world['kind']),
@@ -298,13 +314,14 @@ def fleet_csr(robot_world, W):
 
 
 def convert_fleet_obstacles_batch(world, state, robot_world, fleet, N, T, E, dt, time_varying=False, order=True,
-                                  plan=False):
+                                  plan=False, ids=False):
     """convert_world_obstacles_batch with the robots as obstacles of each other: robot b chooses from every shape of
     its world followed by every other robot of its world in ascending index, fleet [m] being robot m's shape (from
     fleet_shapes_batch).  robot_world [B] int32 or None (every robot in world 0).  Returns obs_A [B,N,Tc,E,2], obs_b [B,N,Tc,E], obs_kind [B,N], obs_count [B] (world
     size plus the robots of the world minus one).  plan: the stage-t copy of a mate is its body along its plan,
     fleet['plan_xy'][m, t] (from fleet_plan_shapes_batch), instead of its shape moved at constant velocity; the same
-    slots in the same order.  Needs time_varying."""
+    slots in the same order.  Needs time_varying.  ids: also returns obs_id [B,N] int32, each slot's obstacle: the flat
+    index of a world shape, S + m for map-mate robot m (S the number of packed shapes), -1 for an empty list."""
     if plan and not time_varying:
         raise ValueError('a fleet predicted along its plans needs time_varying=True')
     lib = _cabi.load()
@@ -322,6 +339,11 @@ def convert_fleet_obstacles_batch(world, state, robot_world, fleet, N, T, E, dt,
             _ptr(fleet['vel']))
     outs = (_ptr(A), _ptr(b), _ptr(kind), _ptr(count), _stream(dev))
     with torch.cuda.device(dev):
+        if ids:
+            obs_id = torch.empty((B, N), dtype=torch.int32, device=dev)
+            _cabi.check(lib.rda_convert_world_obstacles_ids(*args, _ptr(fleet['plan_xy']) if plan else None, *outs[:4],
+                                                            _ptr(obs_id), outs[4]), 'rda_convert_world_obstacles_ids')
+            return A, b, kind, count, obs_id
         if plan:
             _cabi.check(lib.rda_convert_fleet_plan_obstacles(*args, _ptr(fleet['plan_xy']), *outs),
                         'rda_convert_fleet_plan_obstacles')
@@ -331,13 +353,14 @@ def convert_fleet_obstacles_batch(world, state, robot_world, fleet, N, T, E, dt,
 
 
 def convert_world_obstacles_horizon_batch(world, nom_s, ref_s, body, robot_world, N, T, E, dt, time_varying=False,
-                                          fleet=None, plan=False, per_robot=None):
+                                          fleet=None, plan=False, per_robot=None, ids=False):
     """convert_world_obstacles_batch (fleet None) or convert_fleet_obstacles_batch (fleet from fleet_shapes_batch or,
     with plan, fleet_plan_shapes_batch) in the horizon order: each robot's shapes sorted by the smallest signed distance
     between its body and the shape's rows over its nominal and reference poses, nom_s, ref_s [B,3,T+1] CUDA tensors.
     body from robot_body with xy a CUDA tensor; per_robot None, or a dict with CUDA tensors 'xy' [B,8,2] and 'radius'
     [B], each robot's own body (body gives the kind and vertex count).  The same list, padding, outputs and obs_count
-    as those calls; without a host synchronisation."""
+    as those calls; without a host synchronisation.  ids: also returns obs_id [B,N] int32, the ids of
+    convert_fleet_obstacles_batch."""
     if plan and (fleet is None or not time_varying):
         raise ValueError('a fleet predicted along its plans needs a fleet and time_varying=True')
     lib = _cabi.load()
@@ -354,13 +377,17 @@ def convert_world_obstacles_horizon_batch(world, nom_s, ref_s, body, robot_world
         mates = (_ptr(csr[0]), _ptr(csr[1]), _ptr(fleet['kind']), _ptr(fleet['nv']), _ptr(fleet['xy']),
                  _ptr(fleet['radius']), _ptr(fleet['vel']), _ptr(fleet['plan_xy']) if plan else None)
     pr = per_robot or {}
-    with torch.cuda.device(dev):
-        _cabi.check(lib.rda_convert_world_obstacles_horizon(
-            B, W, N, T, E, dt, int(time_varying), _ptr(nom_s), _ptr(ref_s), int(body['kind']), int(body['nv']),
+    args = (B, W, N, T, E, dt, int(time_varying), _ptr(nom_s), _ptr(ref_s), int(body['kind']), int(body['nv']),
             _ptr(body['xy']), float(body['radius']), _ptr(pr.get('xy')), _ptr(pr.get('radius')), _ptr(world['start']),
             _ptr(robot_world), _ptr(world['kind']), _ptr(world['nv']), _ptr(world['xy']), _ptr(world['radius']),
-            _ptr(world['vel']), *mates, _ptr(A), _ptr(b), _ptr(kind), _ptr(count), _stream(dev)),
-            'rda_convert_world_obstacles_horizon')
+            _ptr(world['vel']), *mates, _ptr(A), _ptr(b), _ptr(kind), _ptr(count))
+    with torch.cuda.device(dev):
+        if ids:
+            obs_id = torch.empty((B, N), dtype=torch.int32, device=dev)
+            _cabi.check(lib.rda_convert_world_obstacles_horizon_ids(*args, _ptr(obs_id), _stream(dev)),
+                        'rda_convert_world_obstacles_horizon_ids')
+            return A, b, kind, count, obs_id
+        _cabi.check(lib.rda_convert_world_obstacles_horizon(*args, _stream(dev)), 'rda_convert_world_obstacles_horizon')
     return A, b, kind, count
 
 
@@ -398,13 +425,23 @@ class BatchedMPC:
     position to a polygon's nearest vertex or a disc's centre), False keeps list order, and 'horizon' sorts them by how
     close the robot's horizon comes to them: the smallest signed distance between its body and the obstacle's rows over
     its nominal and reference poses (convert_world_obstacles_horizon_batch).  'horizon' takes world= (and avoid_fleet),
-    not shapes=."""
+    not shapes=.
+
+    warm_start: 'slot' (default, the reference's behaviour) leaves each slot's warm start (the ADMM multipliers of the
+    last solve) in its slot, whichever obstacle the selection puts there next; 'obstacle' moves it with the obstacle
+    (RDA_solver.set_obstacle_ids), and info['obs_id'] [B,N] says which obstacle each slot held.  An obstacle's identity
+    is its list position: its flat index in the packed world (pack_worlds), S + m for map-mate robot m (S packed shapes),
+    its position in a robot's shapes= list.  A caller who repacks a map must keep its order for the warm start to
+    follow.  A step without obstacles gives every slot the id -1, so each slot starts cold when obstacles come back."""
 
     def __init__(self, car_tuple, ref_path, batch, receding=10, sample_time=0.1, iter_num=4,
                  enable_reverse=False, obstacle_order=True, max_edge_num=5, max_obs_num=5,
                  accelerated=True, goal_index_threshold=1, device=None, iter_threshold=0.2, robot_path=None,
-                 robot_class=None, **kwargs):
+                 robot_class=None, warm_start='slot', **kwargs):
         self.lib = _cabi.load()
+        if warm_start not in ('slot', 'obstacle'):
+            raise ValueError(f"warm_start is 'slot' or 'obstacle', not {warm_start!r}")
+        self.warm_start = warm_start
         self.enable_reverse = bool(enable_reverse)
         self.classes = None
         if robot_class is not None:
@@ -580,8 +617,9 @@ class BatchedMPC:
                     B, T, _ptr(self.per_robot['dynamics']), self.dt, _ptr(self.per_robot['wheelbase']), _ptr(state),
                     _ptr(self.cur_vel), _ptr(ref_speed), *paths), 'rda_pre_process_paths_per_robot')
         self.cur_index = near
+        ids = self.warm_start == 'obstacle'
         if (shapes is None and world is None) or self.N == 0:
-            A, b, kind, count = self._no_obstacles()
+            conv = self._no_obstacles() + ((torch.full((B, self.N), -1, dtype=torch.int32, device=dev),) if ids else ())
             time_varying = False
         elif horizon:
             fleet = None
@@ -589,23 +627,26 @@ class BatchedMPC:
                 fleet = fleet_shapes_batch(state, self.cur_vel, self.body, self.dynamics, self.per_robot) if not plan \
                     else fleet_plan_shapes_batch(state, self.cur_vel, self.body, self.dynamics, self.dt, self.L,
                                                  self.per_robot)
-            A, b, kind, count = convert_world_obstacles_horizon_batch(world, nom_s, ref_s, self.body, robot_world, self.N,
-                                                                      T, self.E, self.dt, time_varying, fleet, plan,
-                                                                      self.per_robot)
+            conv = convert_world_obstacles_horizon_batch(world, nom_s, ref_s, self.body, robot_world, self.N, T, self.E,
+                                                         self.dt, time_varying, fleet, plan, self.per_robot, ids)
         elif avoid_fleet:
             if plan:
                 fleet = fleet_plan_shapes_batch(state, self.cur_vel, self.body, self.dynamics, self.dt, self.L,
                                                 self.per_robot)
             else:
                 fleet = fleet_shapes_batch(state, self.cur_vel, self.body, self.dynamics, self.per_robot)
-            A, b, kind, count = convert_fleet_obstacles_batch(world, state, robot_world, fleet, self.N, T, self.E,
-                                                              self.dt, time_varying, self.obstacle_order, plan)
+            conv = convert_fleet_obstacles_batch(world, state, robot_world, fleet, self.N, T, self.E, self.dt,
+                                                 time_varying, self.obstacle_order, plan, ids)
         elif world is not None:
-            A, b, kind, count = convert_world_obstacles_batch(world, state, robot_world, self.N, T, self.E, self.dt,
-                                                              time_varying, self.obstacle_order)
+            conv = convert_world_obstacles_batch(world, state, robot_world, self.N, T, self.E, self.dt, time_varying,
+                                                 self.obstacle_order, ids)
         else:
-            A, b, kind, count = convert_obstacles_batch(shapes, state, self.N, T, self.E, self.dt, time_varying,
-                                                        self.obstacle_order)
+            conv = convert_obstacles_batch(shapes, state, self.N, T, self.E, self.dt, time_varying, self.obstacle_order,
+                                           ids)
+        A, b, kind, count = conv[:4]
+        obs_id = conv[4] if ids else None
+        if ids:
+            self.rda.set_obstacle_ids(obs_id)
         out = self.rda.iterative_solve_batch(nom_s, self.cur_vel, ref_s, solver_speed, A, b, kind, count, time_varying)
         with torch.cuda.device(dev):
             _cabi.check(self.lib.rda_post_process_paths(B, T, self.n_paths, _ptr(self.path_curve), _ptr(self.curve_start),
@@ -614,6 +655,8 @@ class BatchedMPC:
                                                         _ptr(self.arrive), _stream(dev)), 'rda_post_process_paths')
         info = dict(out)
         info.update(arrive=self.arrive, nom_s=nom_s, ref_s=ref_s, cur_index=near, curve_index=self.curve_index)
+        if ids:
+            info['obs_id'] = obs_id
         if clearance:
             c = self.rda.plan_clearance()
             info.update(clearance=c['min'], clearance_index=c['index'])

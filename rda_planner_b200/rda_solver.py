@@ -546,6 +546,27 @@ class RDA_solver:
         self._class_index = index   # the copy into the handle's storage reads it on the current stream
         self._apply_class_limits(index, None if previous is None else self.class_slot(index) != self.class_slot(previous))
 
+    # ------------------------------------------------------------------ warm start that follows the obstacles
+    def set_obstacle_ids(self, ids):
+        """ids [B, N] (array-like or CUDA tensor, int32 values; < 0: no obstacle): the obstacle each slot holds in the next
+        solve, as the *_batch conversions return them with ids=True.  When ids of an earlier call are held, each
+        instance's per-slot warm start (lam, mu, z, xi, zeta and the su-QP coefficients) moves with its obstacles: the
+        k-th slot carrying id X takes the state of the k-th slot that carried X; a slot without a match starts cold.
+        The first call only stores the ids; None forgets them (the reference's behaviour: the state stays in its slot).
+        reset() and cold_start() keep them.  One kernel on the current stream, no host synchronisation."""
+        with torch.cuda.device(self.device):
+            if ids is None:
+                _cabi.check(self.lib.rda_set_obstacle_ids(self._h, None, self._stream()), 'rda_set_obstacle_ids')
+                self._keep_ids = None
+                return
+            t = torch.as_tensor(ids, device=self.device).to(torch.int32).reshape(self.batch, self.max_obs_num)
+            t = t.contiguous()
+            if self.max_obs_num == 0:
+                return
+            _cabi.check(self.lib.rda_set_obstacle_ids(self._h, C.c_void_p(t.data_ptr()), self._stream()),
+                        'rda_set_obstacle_ids')
+            self._keep_ids = t          # read asynchronously on the current stream
+
     def get_adjust_parameter(self):
         t = _cabi.Tunables()
         _cabi.check(self.lib.rda_get_tunables(self._h, C.byref(t)), 'rda_get_tunables')
