@@ -393,6 +393,48 @@ int rda_convert_world_obstacles_horizon_ids(int B, int W, int N, int T, int E, f
                                             float *obs_b, int32_t *obs_kind, int32_t *obs_count, int32_t *obs_id,
                                             void *cuda_stream);
 
+/* WORLD SHAPES ALONG TRAJECTORIES: a world shape may follow a given trajectory over the horizon (a predictor's output
+ * for a pedestrian, a vehicle, a forklift) instead of standing still or translating at its constant velocity.  In the
+ * reference's terms such a shape is rdaobs(A = [A_0 .. A_T], b = [b_0 .. b_T]) of its stage shapes (MPC(rda_obstacle=
+ * True), rda_solver.py:501-526).  The two calls take the arguments of rda_convert_world_obstacles_ids /
+ * rda_convert_world_obstacles_horizon_ids (fleet_start = NULL: no fleet; fleet_plan_xy = NULL: mates at constant
+ * velocity; obs_id = NULL: no ids) plus the trajectory table (device):
+ *   shape_traj int32 [S]: the trajectory of each packed shape; a value outside [0, K) means none (the shape's own
+ *   shape_xy and shape_vel, exactly as the calls above; decided on the device);
+ *   traj_xy float32 [K][T+1][RDA_MAX_EDGE][2], 16-byte aligned: trajectory k's shape at stage t in the world frame,
+ *   a polygon's shape_nv vertices (either orientation, as shape_xy) or a disc's centre in row 0 (the radius stays
+ *   shape_radius).
+ * For a shape with trajectory k, traj_xy[k] replaces its shape_xy and shape_vel everywhere: its stage-t rows are
+ * obstacle rows of traj_xy[k][t] standing still (no velocity threshold), its reference key (order != 0) is taken from
+ * traj_xy[k][0], and its horizon key uses its stage-t rows.  It gets no one-disc bound in the horizon order, only the
+ * bound of every pose.  Slots, padding, obs_kind, obs_count and ids (the flat shape index) keep their meaning.  Both
+ * arrays may be rewritten on the device between calls; a captured graph reads the new values on replay.
+ * Usage errors are return codes: RDA_E_ARG for NULL shape_traj or traj_xy, an unaligned traj_xy, K < 1 or
+ * time_varying == 0 (a trajectory has T+1 copies); the rest as in the calls they extend.  No allocation, host sync or
+ * graph break. */
+int rda_convert_world_obstacles_traj(int B, int W, int N, int T, int E, float dt, int time_varying, int order,
+                                     const float *state, const int32_t *world_start, const int32_t *robot_world,
+                                     const int32_t *shape_kind, const int32_t *shape_nv, const float *shape_xy,
+                                     const float *shape_radius, const float *shape_vel, const int32_t *fleet_start,
+                                     const int32_t *fleet_robot, const int32_t *fleet_kind, const int32_t *fleet_nv,
+                                     const float *fleet_xy, const float *fleet_radius, const float *fleet_vel,
+                                     const float *fleet_plan_xy, float *obs_A, float *obs_b, int32_t *obs_kind,
+                                     int32_t *obs_count, int32_t *obs_id, const int32_t *shape_traj, int K,
+                                     const float *traj_xy, void *cuda_stream);
+int rda_convert_world_obstacles_horizon_traj(int B, int W, int N, int T, int E, float dt, int time_varying,
+                                             const float *nom_s, const float *ref_s, int body_kind, int body_nv,
+                                             const float *body_xy, float body_radius, const float *body_xy_b,
+                                             const float *body_radius_b, const int32_t *world_start,
+                                             const int32_t *robot_world, const int32_t *shape_kind,
+                                             const int32_t *shape_nv, const float *shape_xy, const float *shape_radius,
+                                             const float *shape_vel, const int32_t *fleet_start,
+                                             const int32_t *fleet_robot, const int32_t *fleet_kind,
+                                             const int32_t *fleet_nv, const float *fleet_xy, const float *fleet_radius,
+                                             const float *fleet_vel, const float *fleet_plan_xy, float *obs_A,
+                                             float *obs_b, int32_t *obs_kind, int32_t *obs_count, int32_t *obs_id,
+                                             const int32_t *shape_traj, int K, const float *traj_xy,
+                                             void *cuda_stream);
+
 /* Arrive rule of MPC.control (mpc.py:170-185, single gear): instances whose near_index >=
  * P - goal_index_threshold get u_opt = 0 and arrive = 1; cur_vel (may be NULL) receives the
  * controls kept as the next step's nominal (mpc.py:186).  u_opt, cur_vel [B][2][T].        */

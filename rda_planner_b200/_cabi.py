@@ -64,7 +64,8 @@ EXPORTS = ['rda_create', 'rda_destroy', 'rda_set_tunables', 'rda_get_tunables', 
            'rda_pre_process_paths_per_robot', 'rda_motion_predict_per_robot', 'rda_fleet_shapes_per_robot',
            'rda_plan_clearance', 'rda_fleet_plan_shapes', 'rda_convert_fleet_plan_obstacles',
            'rda_convert_world_obstacles_horizon', 'rda_set_obstacle_ids', 'rda_convert_obstacles_ids',
-           'rda_convert_world_obstacles_ids', 'rda_convert_world_obstacles_horizon_ids']
+           'rda_convert_world_obstacles_ids', 'rda_convert_world_obstacles_horizon_ids',
+           'rda_convert_world_obstacles_traj', 'rda_convert_world_obstacles_horizon_traj']
 MAX_SHAPES = 64
 MAX_WORLD_SLOTS = 256
 
@@ -126,6 +127,9 @@ def load():
     lib.rda_convert_obstacles_ids.argtypes = [i, i, i, i, i, f, i, i] + [vp] * 13
     lib.rda_convert_world_obstacles_ids.argtypes = [i, i, i, i, i, f, i, i] + [vp] * 22
     lib.rda_convert_world_obstacles_horizon_ids.argtypes = [i, i, i, i, i, f, i, vp, vp, i, i, vp, f] + [vp] * 23
+    lib.rda_convert_world_obstacles_traj.argtypes = [i, i, i, i, i, f, i, i] + [vp] * 21 + [vp, i, vp, vp]
+    lib.rda_convert_world_obstacles_horizon_traj.argtypes = ([i, i, i, i, i, f, i, vp, vp, i, i, vp, f] + [vp] * 22 +
+                                                             [vp, i, vp, vp])
     for name in EXPORTS:
         if name != 'rda_version':
             getattr(lib, name).restype = C.c_int

@@ -181,16 +181,32 @@ __device__ __forceinline__ void world_merge(int tid, int c, int N, double* kkey,
   __syncthreads();
 }
 
+// The trajectory of world shape s: its stages traj_xy [k][0..T] ([T+1][RDA_MAX_EDGE][2] each) when k = shape_traj[s]
+// is in [0, K), else NULL (the shape's own xy and vel).
+__device__ __forceinline__ const float* world_traj(const int* shape_traj, int K, const float* traj_xy, int T1, size_t s) {
+  const int k = shape_traj[s];
+  return k >= 0 && k < K ? traj_xy + (size_t)k * T1 * RDA_MAX_EDGE * 2 : nullptr;
+}
+
+// The current shape of world shape s: stage 0 of its trajectory, else its own xy.
+__device__ __forceinline__ const float* world_xy0(const int* shape_traj, int K, const float* traj_xy, int T1,
+                                                  const float* shape_xy, size_t s) {
+  const float* tr = world_traj(shape_traj, K, traj_xy, T1, s);
+  return tr ? tr : shape_xy + s * RDA_MAX_EDGE * 2;
+}
+
 // The rows of the N slots of robot b: slot n is the list entry kept_idx[n] (list order when kept_idx is NULL), the
 // last one repeated past the list, all-zero rows for an empty list.  kPlan: map-mates are read along fleet_plan_xy.
-template <bool kPlan>
+// kTraj: world shapes with a trajectory (world_traj) are read along it (time-varying output only).
+template <bool kPlan, bool kTraj>
 __device__ __forceinline__ void world_slots(int tid, int b, int B, int N, int T, int E, float dt, int time_varying,
                                             int count, const ShapeList& L, const int* kept_idx, const int* shape_kind,
                                             const int* shape_nv, const float* shape_xy, const float* shape_radius,
                                             const float* shape_vel, const int* fleet_robot, const int* fleet_kind,
                                             const int* fleet_nv, const float* fleet_xy, const float* fleet_radius,
                                             const float* fleet_vel, const float* fleet_plan_xy, float* obs_A,
-                                            float* obs_b, int* obs_kind) {
+                                            float* obs_b, int* obs_kind, const int* shape_traj, int K,
+                                            const float* traj_xy) {
   const int Tc = time_varying ? T + 1 : 1;
   for (int q = tid; q < N * Tc; q += kWorldTile) {     // one (slot, stage) copy per thread
     const int n = q / Tc, t = q - n * Tc;
@@ -210,8 +226,11 @@ __device__ __forceinline__ void world_slots(int tid, int b, int B, int N, int T,
     if (t == 0) obs_kind[(size_t)b * N + n] = kind;
     const float* xy = (mate ? fleet_xy : shape_xy) + s * RDA_MAX_EDGE * 2;
     double vx = 0.0, vy = 0.0;
+    const float* tr = kTraj && !mate ? world_traj(shape_traj, K, traj_xy, T + 1, s) : nullptr;
     if (kPlan && mate) {                               // a map-mate along its plan: its stage-t shape, standing
       xy = fleet_plan_xy + (s * (T + 1) + t) * RDA_MAX_EDGE * 2;
+    } else if (kTraj && tr) {                          // a world shape along its trajectory: likewise
+      xy = tr + (size_t)t * RDA_MAX_EDGE * 2;
     } else {
       const float* vel = (mate ? fleet_vel : shape_vel) + 2 * s;
       vx = vel[0]; vy = vel[1];
@@ -241,7 +260,9 @@ __device__ __forceinline__ void world_slot_ids(int tid, int b, int B, int N, int
 // kPlan: map-mates are read along their plans, fleet_plan_xy [B][T+1][RDA_MAX_EDGE][2] (time-varying output only);
 // the variant without plans never reads it, and compiles to the code it had before plans existed.
 // kIds: also the slots' obstacle ids (world_slots) into obs_id.
-template <bool kPlan, bool kIds>
+// kTraj: world shapes with a trajectory are keyed by its stage 0 and written along it (world_traj; time-varying output
+// only); the variant without never reads shape_traj / traj_xy, and compiles to the code it had before trajectories.
+template <bool kPlan, bool kIds, bool kTraj>
 __device__ __forceinline__ void convert_world(int B, int W, int N, int T, int E, float dt, int time_varying, int order,
                                               const float* state, const int* world_start, const int* robot_world,
                                               const int* shape_kind, const int* shape_nv, const float* shape_xy,
@@ -249,7 +270,8 @@ __device__ __forceinline__ void convert_world(int B, int W, int N, int T, int E,
                                               const int* fleet_robot, const int* fleet_kind, const int* fleet_nv,
                                               const float* fleet_xy, const float* fleet_radius, const float* fleet_vel,
                                               const float* fleet_plan_xy, float* obs_A, float* obs_b, int* obs_kind,
-                                              int* obs_count, int* obs_id) {
+                                              int* obs_count, int* obs_id, const int* shape_traj, int K,
+                                              const float* traj_xy) {
   // dynamic shared memory (order != 0): kept keys [2][N], candidate keys [2][tile], kept indices [2][N],
   // candidate indices [2][tile]; the kept list is double-buffered, candidates are gathered then sorted
   extern __shared__ double sh[];
@@ -289,7 +311,9 @@ __device__ __forceinline__ void convert_world(int B, int W, int N, int T, int E,
         bool mate;
         const size_t s = list_entry(L, i, fleet_robot, b, B, &mate);
         const double key = obstacle_key((mate ? fleet_kind : shape_kind)[s], (mate ? fleet_nv : shape_nv)[s],
-                                        (mate ? fleet_xy : shape_xy) + s * RDA_MAX_EDGE * 2, sx, sy);
+                                        kTraj && !mate ? world_xy0(shape_traj, K, traj_xy, T + 1, shape_xy, s)
+                                                       : (mate ? fleet_xy : shape_xy) + s * RDA_MAX_EDGE * 2,
+                                        sx, sy);
         if (nk < N || key < kkey[cur * N + N - 1]) {
           const int p = atomicAdd(&n_cand[tile], 1);
           ckey[p] = key; cidx[p] = i;
@@ -306,9 +330,9 @@ __device__ __forceinline__ void convert_world(int B, int W, int N, int T, int E,
     kept_idx = kidx + cur * N;
   }
   if (tid == 0) obs_count[b] = count;
-  world_slots<kPlan>(tid, b, B, N, T, E, dt, time_varying, count, L, kept_idx, shape_kind, shape_nv, shape_xy,
-                     shape_radius, shape_vel, fleet_robot, fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel,
-                     fleet_plan_xy, obs_A, obs_b, obs_kind);
+  world_slots<kPlan, kTraj>(tid, b, B, N, T, E, dt, time_varying, count, L, kept_idx, shape_kind, shape_nv, shape_xy,
+                            shape_radius, shape_vel, fleet_robot, fleet_kind, fleet_nv, fleet_xy, fleet_radius,
+                            fleet_vel, fleet_plan_xy, obs_A, obs_b, obs_kind, shape_traj, K, traj_xy);
   if (kIds) world_slot_ids(tid, b, B, N, count, L, kept_idx, fleet_robot, world_start[W], obs_id);
 }
 
@@ -326,13 +350,18 @@ __device__ __forceinline__ void convert_world(int B, int W, int N, int T, int E,
       shape_vel, fleet_start, fleet_robot, fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel, fleet_plan_xy,      \
       obs_A, obs_b, obs_kind, obs_count
 
-template <bool kPlan>
-__global__ void __launch_bounds__(kWorldTile) k_convert_world_obstacles(RDA_WORLD_PARAMS) {
-  convert_world<kPlan, false>(RDA_WORLD_ARGS, nullptr);
+// The trajectory table (kTraj), last so that the parameters before it keep their offsets in every variant
+#define RDA_TRAJ_PARAMS const int *shape_traj, int K, const float *traj_xy
+#define RDA_TRAJ_ARGS shape_traj, K, traj_xy
+
+template <bool kPlan, bool kTraj>
+__global__ void __launch_bounds__(kWorldTile) k_convert_world_obstacles(RDA_WORLD_PARAMS, RDA_TRAJ_PARAMS) {
+  convert_world<kPlan, false, kTraj>(RDA_WORLD_ARGS, nullptr, RDA_TRAJ_ARGS);
 }
-template <bool kPlan>
-__global__ void __launch_bounds__(kWorldTile) k_convert_world_obstacles_ids(RDA_WORLD_PARAMS, int* obs_id) {
-  convert_world<kPlan, true>(RDA_WORLD_ARGS, obs_id);
+template <bool kPlan, bool kTraj>
+__global__ void __launch_bounds__(kWorldTile) k_convert_world_obstacles_ids(RDA_WORLD_PARAMS, int* obs_id,
+                                                                             RDA_TRAJ_PARAMS) {
+  convert_world<kPlan, true, kTraj>(RDA_WORLD_ARGS, obs_id, RDA_TRAJ_ARGS);
 }
 
 // Horizon order (rda_convert_world_obstacles_horizon): the tiles, candidates and merge of k_convert_world_obstacles
@@ -360,8 +389,8 @@ __global__ void __launch_bounds__(kWorldTile) k_convert_world_obstacles_ids(RDA_
       world_start, robot_world, shape_kind, shape_nv, shape_xy, shape_radius, shape_vel, fleet_start, fleet_robot,      \
       fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel, fleet_plan_xy, obs_A, obs_b, obs_kind, obs_count
 
-template <int EC, int RC, bool kPlan, bool kIds>
-__device__ __forceinline__ void convert_world_horizon(RDA_HORIZON_PARAMS, int* obs_id) {
+template <int EC, int RC, bool kPlan, bool kIds, bool kTraj>
+__device__ __forceinline__ void convert_world_horizon(RDA_HORIZON_PARAMS, int* obs_id, RDA_TRAJ_PARAMS) {
   // dynamic shared memory: as k_convert_world_obstacles, then the survivors of a tile [tile]
   extern __shared__ double sh[];
   __shared__ int n_surv, n_cand;
@@ -418,7 +447,8 @@ __device__ __forceinline__ void convert_world_horizon(RDA_HORIZON_PARAMS, int* o
           const RawShape r = {(mate ? fleet_kind : shape_kind)[s], (mate ? fleet_nv : shape_nv)[s],
                               (mate ? fleet_xy : shape_xy) + s * RDA_MAX_EDGE * 2,
                               (double)(mate ? fleet_radius : shape_radius)[s], (double)vel[0], (double)vel[1],
-                              kPlan && mate ? fleet_plan_xy + s * T1 * RDA_MAX_EDGE * 2 : nullptr};
+                              kPlan && mate ? fleet_plan_xy + s * T1 * RDA_MAX_EDGE * 2
+                              : kTraj && !mate ? world_traj(shape_traj, K, traj_xy, T1, s) : nullptr};
           keep = horizon_disc_bound(r, time_varying, T, dtd, E, hor[0], hor[1], hor[2], hor[3]) < thr &&
                  horizon_bound(r, time_varying, T, dtd, E, nom, ref, hor[3], thr) < thr;
         }
@@ -434,7 +464,8 @@ __device__ __forceinline__ void convert_world_horizon(RDA_HORIZON_PARAMS, int* o
         const RawShape r = {(mate ? fleet_kind : shape_kind)[s], (mate ? fleet_nv : shape_nv)[s],
                             (mate ? fleet_xy : shape_xy) + s * RDA_MAX_EDGE * 2,
                             (double)(mate ? fleet_radius : shape_radius)[s], (double)vel[0], (double)vel[1],
-                            kPlan && mate ? fleet_plan_xy + s * T1 * RDA_MAX_EDGE * 2 : nullptr};
+                            kPlan && mate ? fleet_plan_xy + s * T1 * RDA_MAX_EDGE * 2
+                            : kTraj && !mate ? world_traj(shape_traj, K, traj_xy, T1, s) : nullptr};
         double key = INFINITY;
         for (int q = lane; q < 2 * T1; q += 32) {
           const float* p = q < T1 ? nom : ref;
@@ -459,19 +490,20 @@ __device__ __forceinline__ void convert_world_horizon(RDA_HORIZON_PARAMS, int* o
     kept_idx = kidx + cur * N;
   }
   if (tid == 0) obs_count[b] = count;
-  world_slots<kPlan>(tid, b, B, N, T, E, dt, time_varying, count, L, kept_idx, shape_kind, shape_nv, shape_xy,
-                     shape_radius, shape_vel, fleet_robot, fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel,
-                     fleet_plan_xy, obs_A, obs_b, obs_kind);
+  world_slots<kPlan, kTraj>(tid, b, B, N, T, E, dt, time_varying, count, L, kept_idx, shape_kind, shape_nv, shape_xy,
+                            shape_radius, shape_vel, fleet_robot, fleet_kind, fleet_nv, fleet_xy, fleet_radius,
+                            fleet_vel, fleet_plan_xy, obs_A, obs_b, obs_kind, shape_traj, K, traj_xy);
   if (kIds) world_slot_ids(tid, b, B, N, count, L, kept_idx, fleet_robot, world_start[W], obs_id);
 }
 
-template <int EC, int RC, bool kPlan>
-__global__ void __launch_bounds__(kWorldTile) k_convert_world_obstacles_horizon(RDA_HORIZON_PARAMS) {
-  convert_world_horizon<EC, RC, kPlan, false>(RDA_HORIZON_ARGS, nullptr);
+template <int EC, int RC, bool kPlan, bool kTraj>
+__global__ void __launch_bounds__(kWorldTile) k_convert_world_obstacles_horizon(RDA_HORIZON_PARAMS, RDA_TRAJ_PARAMS) {
+  convert_world_horizon<EC, RC, kPlan, false, kTraj>(RDA_HORIZON_ARGS, nullptr, RDA_TRAJ_ARGS);
 }
-template <int EC, int RC, bool kPlan>
-__global__ void __launch_bounds__(kWorldTile) k_convert_world_obstacles_horizon_ids(RDA_HORIZON_PARAMS, int* obs_id) {
-  convert_world_horizon<EC, RC, kPlan, true>(RDA_HORIZON_ARGS, obs_id);
+template <int EC, int RC, bool kPlan, bool kTraj>
+__global__ void __launch_bounds__(kWorldTile) k_convert_world_obstacles_horizon_ids(RDA_HORIZON_PARAMS, int* obs_id,
+                                                                                     RDA_TRAJ_PARAMS) {
+  convert_world_horizon<EC, RC, kPlan, true, kTraj>(RDA_HORIZON_ARGS, obs_id, RDA_TRAJ_ARGS);
 }
 
 // Each robot of a fleet as a raw shape for its map-mates (fleet_shape), one thread per robot: its body at its pose,
@@ -543,16 +575,24 @@ __global__ void k_motion_predict(int B, int T, int dynamics, float dt, float L, 
   state[3 * b] = (float)o[0]; state[3 * b + 1] = (float)o[1]; state[3 * b + 2] = (float)o[2];
 }
 
+// The checks of the trajectory table (traj: the _traj entry points): both arrays, traj_xy 16-byte aligned, K >= 1 and
+// time-varying output.
+bool traj_args_ok(bool traj, int time_varying, const int32_t* shape_traj, int K, const float* traj_xy) {
+  return !traj || (shape_traj && traj_xy && !((uintptr_t)traj_xy & 15) && K >= 1 && time_varying);
+}
+
 // Argument checks and launch of k_convert_world_obstacles.  Without `fleet` the fleet pointers are NULL and each robot
-// chooses from its world's shapes only; fleet_plan_xy (fleet only, time-varying output only) may be NULL.
-int launch_world_obstacles(bool fleet, int B, int W, int N, int T, int E, float dt, int time_varying, int order,
+// chooses from its world's shapes only; fleet_plan_xy (fleet only, time-varying output only) may be NULL.  With `traj`
+// world shapes may follow the trajectories of (shape_traj, K, traj_xy); without, those are not read.
+int launch_world_obstacles(bool fleet, bool traj, int B, int W, int N, int T, int E, float dt, int time_varying, int order,
                            const float* state, const int32_t* world_start, const int32_t* robot_world,
                            const int32_t* shape_kind, const int32_t* shape_nv, const float* shape_xy,
                            const float* shape_radius, const float* shape_vel, const int32_t* fleet_start,
                            const int32_t* fleet_robot, const int32_t* fleet_kind, const int32_t* fleet_nv,
                            const float* fleet_xy, const float* fleet_radius, const float* fleet_vel,
                            const float* fleet_plan_xy, float* obs_A, float* obs_b, int32_t* obs_kind,
-                           int32_t* obs_count, int32_t* obs_id, cudaStream_t stream) {
+                           int32_t* obs_count, int32_t* obs_id, const int32_t* shape_traj, int K,
+                           const float* traj_xy, cudaStream_t stream) {
   if (B < 1 || W < 1 || N < 1 || T < 1) return RDA_E_ARG;
   if (N > RDA_MAX_WORLD_SLOTS || E < 3 || E > RDA_MAX_EDGE) return RDA_E_UNSUPPORTED;
   if (!world_start || !shape_kind || !shape_nv || !shape_xy || !shape_radius || !shape_vel) return RDA_E_ARG;
@@ -560,20 +600,26 @@ int launch_world_obstacles(bool fleet, int B, int W, int N, int T, int E, float 
   if (fleet && (!fleet_start || !fleet_robot || !fleet_kind || !fleet_nv || !fleet_xy || !fleet_radius || !fleet_vel))
     return RDA_E_ARG;
   if (fleet_plan_xy && (!fleet || !time_varying)) return RDA_E_ARG;
+  if (!traj_args_ok(traj, time_varying, shape_traj, K, traj_xy)) return RDA_E_ARG;
   const size_t smem = order ? (size_t)(2 * N + 2 * kWorldTile) * (sizeof(double) + sizeof(int)) : 0;
-  if (obs_id)
-    (fleet_plan_xy ? k_convert_world_obstacles_ids<true> : k_convert_world_obstacles_ids<false>)<<<B, kWorldTile, smem, stream>>>(
-        RDA_WORLD_ARGS, obs_id);
-  else
-    (fleet_plan_xy ? k_convert_world_obstacles<true> : k_convert_world_obstacles<false>)<<<B, kWorldTile, smem, stream>>>(
-        RDA_WORLD_ARGS);
+  const bool plan = fleet_plan_xy != nullptr;
+  if (obs_id) {
+    auto k = traj ? (plan ? k_convert_world_obstacles_ids<true, true> : k_convert_world_obstacles_ids<false, true>)
+                  : (plan ? k_convert_world_obstacles_ids<true, false> : k_convert_world_obstacles_ids<false, false>);
+    k<<<B, kWorldTile, smem, stream>>>(RDA_WORLD_ARGS, obs_id, RDA_TRAJ_ARGS);
+  } else {
+    auto k = traj ? (plan ? k_convert_world_obstacles<true, true> : k_convert_world_obstacles<false, true>)
+                  : (plan ? k_convert_world_obstacles<true, false> : k_convert_world_obstacles<false, false>);
+    k<<<B, kWorldTile, smem, stream>>>(RDA_WORLD_ARGS, RDA_TRAJ_ARGS);
+  }
   RDA_CUDA(cudaGetLastError());
   return 0;
 }
 
 // Argument checks and launch of k_convert_world_obstacles_horizon.  fleet_start NULL: no fleet (the other fleet
-// pointers are then not read); fleet_plan_xy (fleet only, time-varying output only) may be NULL.
-int launch_world_obstacles_horizon(int B, int W, int N, int T, int E, float dt, int time_varying, const float* nom_s,
+// pointers are then not read); fleet_plan_xy (fleet only, time-varying output only) may be NULL; traj as for
+// launch_world_obstacles.
+int launch_world_obstacles_horizon(bool traj, int B, int W, int N, int T, int E, float dt, int time_varying, const float* nom_s,
                                    const float* ref_s, int body_kind, int body_nv, const float* body_xy,
                                    float body_radius, const float* body_xy_b, const float* body_radius_b,
                                    const int32_t* world_start, const int32_t* robot_world, const int32_t* shape_kind,
@@ -582,7 +628,8 @@ int launch_world_obstacles_horizon(int B, int W, int N, int T, int E, float dt, 
                                    const int32_t* fleet_kind, const int32_t* fleet_nv, const float* fleet_xy,
                                    const float* fleet_radius, const float* fleet_vel, const float* fleet_plan_xy,
                                    float* obs_A, float* obs_b, int32_t* obs_kind, int32_t* obs_count,
-                                   int32_t* obs_id, cudaStream_t stream) {
+                                   int32_t* obs_id, const int32_t* shape_traj, int K, const float* traj_xy,
+                                   cudaStream_t stream) {
   if (B < 1 || W < 1 || N < 1 || T < 1) return RDA_E_ARG;
   if (N > RDA_MAX_WORLD_SLOTS || E < 3 || E > RDA_MAX_EDGE) return RDA_E_UNSUPPORTED;
   if (body_kind == RDA_OBS_POLYGON) {
@@ -596,17 +643,30 @@ int launch_world_obstacles_horizon(int B, int W, int N, int T, int E, float dt, 
   const bool fleet = fleet_start != nullptr;
   if (fleet && (!fleet_robot || !fleet_kind || !fleet_nv || !fleet_xy || !fleet_radius || !fleet_vel)) return RDA_E_ARG;
   if (fleet_plan_xy && (!fleet || !time_varying)) return RDA_E_ARG;
+  if (!traj_args_ok(traj, time_varying, shape_traj, K, traj_xy)) return RDA_E_ARG;
   const bool small = E <= 4 && (body_kind == RDA_OBS_CIRCLE || body_nv <= 4);
   const bool plan = fleet_plan_xy != nullptr;
   const size_t smem = (size_t)(2 * N + 2 * kWorldTile) * (sizeof(double) + sizeof(int)) + kWorldTile * sizeof(int);
   if (obs_id) {
-    auto k = small ? (plan ? k_convert_world_obstacles_horizon_ids<4, 4, true> : k_convert_world_obstacles_horizon_ids<4, 4, false>)
-                   : (plan ? k_convert_world_obstacles_horizon_ids<8, 8, true> : k_convert_world_obstacles_horizon_ids<8, 8, false>);
-    k<<<B, kWorldTile, smem, stream>>>(RDA_HORIZON_ARGS, obs_id);
+    auto k = traj ? (small ? (plan ? k_convert_world_obstacles_horizon_ids<4, 4, true, true>
+                                   : k_convert_world_obstacles_horizon_ids<4, 4, false, true>)
+                           : (plan ? k_convert_world_obstacles_horizon_ids<8, 8, true, true>
+                                   : k_convert_world_obstacles_horizon_ids<8, 8, false, true>))
+                  : (small ? (plan ? k_convert_world_obstacles_horizon_ids<4, 4, true, false>
+                                   : k_convert_world_obstacles_horizon_ids<4, 4, false, false>)
+                           : (plan ? k_convert_world_obstacles_horizon_ids<8, 8, true, false>
+                                   : k_convert_world_obstacles_horizon_ids<8, 8, false, false>));
+    k<<<B, kWorldTile, smem, stream>>>(RDA_HORIZON_ARGS, obs_id, RDA_TRAJ_ARGS);
   } else {
-    auto k = small ? (plan ? k_convert_world_obstacles_horizon<4, 4, true> : k_convert_world_obstacles_horizon<4, 4, false>)
-                   : (plan ? k_convert_world_obstacles_horizon<8, 8, true> : k_convert_world_obstacles_horizon<8, 8, false>);
-    k<<<B, kWorldTile, smem, stream>>>(RDA_HORIZON_ARGS);
+    auto k = traj ? (small ? (plan ? k_convert_world_obstacles_horizon<4, 4, true, true>
+                                   : k_convert_world_obstacles_horizon<4, 4, false, true>)
+                           : (plan ? k_convert_world_obstacles_horizon<8, 8, true, true>
+                                   : k_convert_world_obstacles_horizon<8, 8, false, true>))
+                  : (small ? (plan ? k_convert_world_obstacles_horizon<4, 4, true, false>
+                                   : k_convert_world_obstacles_horizon<4, 4, false, false>)
+                           : (plan ? k_convert_world_obstacles_horizon<8, 8, true, false>
+                                   : k_convert_world_obstacles_horizon<8, 8, false, false>));
+    k<<<B, kWorldTile, smem, stream>>>(RDA_HORIZON_ARGS, RDA_TRAJ_ARGS);
   }
   RDA_CUDA(cudaGetLastError());
   return 0;
@@ -616,6 +676,8 @@ int launch_world_obstacles_horizon(int B, int W, int N, int T, int E, float dt, 
 #undef RDA_WORLD_ARGS
 #undef RDA_HORIZON_PARAMS
 #undef RDA_HORIZON_ARGS
+#undef RDA_TRAJ_PARAMS
+#undef RDA_TRAJ_ARGS
 
 }  // namespace
 
@@ -719,10 +781,10 @@ int rda_convert_world_obstacles(int B, int W, int N, int T, int E, float dt, int
                                 const int32_t* shape_kind, const int32_t* shape_nv, const float* shape_xy,
                                 const float* shape_radius, const float* shape_vel, float* obs_A, float* obs_b,
                                 int32_t* obs_kind, int32_t* obs_count, void* stream) {
-  return launch_world_obstacles(false, B, W, N, T, E, dt, time_varying, order, state, world_start, robot_world,
+  return launch_world_obstacles(false, false, B, W, N, T, E, dt, time_varying, order, state, world_start, robot_world,
                                 shape_kind, shape_nv, shape_xy, shape_radius, shape_vel, nullptr, nullptr, nullptr,
                                 nullptr, nullptr, nullptr, nullptr, nullptr, obs_A, obs_b, obs_kind, obs_count,
-                                nullptr, (cudaStream_t)stream);
+                                nullptr, nullptr, 0, nullptr, (cudaStream_t)stream);
 }
 
 int rda_fleet_shapes(int B, int T, int dynamics, int body_kind, int body_nv, const float* body_xy, float body_radius,
@@ -771,10 +833,10 @@ int rda_convert_fleet_obstacles(int B, int W, int N, int T, int E, float dt, int
                                 const int32_t* fleet_robot, const int32_t* fleet_kind, const int32_t* fleet_nv,
                                 const float* fleet_xy, const float* fleet_radius, const float* fleet_vel, float* obs_A,
                                 float* obs_b, int32_t* obs_kind, int32_t* obs_count, void* stream) {
-  return launch_world_obstacles(true, B, W, N, T, E, dt, time_varying, order, state, world_start, robot_world,
+  return launch_world_obstacles(true, false, B, W, N, T, E, dt, time_varying, order, state, world_start, robot_world,
                                 shape_kind, shape_nv, shape_xy, shape_radius, shape_vel, fleet_start, fleet_robot,
                                 fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel, nullptr, obs_A, obs_b,
-                                obs_kind, obs_count, nullptr, (cudaStream_t)stream);
+                                obs_kind, obs_count, nullptr, nullptr, 0, nullptr, (cudaStream_t)stream);
 }
 
 int rda_fleet_plan_shapes(int B, int T, int dynamics, float dt, float wheelbase, int body_kind, int body_nv,
@@ -807,10 +869,10 @@ int rda_convert_fleet_plan_obstacles(int B, int W, int N, int T, int E, float dt
                                      const float* fleet_plan_xy, float* obs_A, float* obs_b, int32_t* obs_kind,
                                      int32_t* obs_count, void* stream) {
   if (!fleet_plan_xy) return RDA_E_ARG;
-  return launch_world_obstacles(true, B, W, N, T, E, dt, time_varying, order, state, world_start, robot_world,
+  return launch_world_obstacles(true, false, B, W, N, T, E, dt, time_varying, order, state, world_start, robot_world,
                                 shape_kind, shape_nv, shape_xy, shape_radius, shape_vel, fleet_start, fleet_robot,
                                 fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel, fleet_plan_xy, obs_A, obs_b,
-                                obs_kind, obs_count, nullptr, (cudaStream_t)stream);
+                                obs_kind, obs_count, nullptr, nullptr, 0, nullptr, (cudaStream_t)stream);
 }
 
 int rda_convert_world_obstacles_horizon(int B, int W, int N, int T, int E, float dt, int time_varying,
@@ -824,11 +886,11 @@ int rda_convert_world_obstacles_horizon(int B, int W, int N, int T, int E, float
                                         const float* fleet_radius, const float* fleet_vel, const float* fleet_plan_xy,
                                         float* obs_A, float* obs_b, int32_t* obs_kind, int32_t* obs_count,
                                         void* stream) {
-  return launch_world_obstacles_horizon(B, W, N, T, E, dt, time_varying, nom_s, ref_s, body_kind, body_nv, body_xy,
+  return launch_world_obstacles_horizon(false, B, W, N, T, E, dt, time_varying, nom_s, ref_s, body_kind, body_nv, body_xy,
                                         body_radius, body_xy_b, body_radius_b, world_start, robot_world, shape_kind,
                                         shape_nv, shape_xy, shape_radius, shape_vel, fleet_start, fleet_robot,
                                         fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel, fleet_plan_xy, obs_A,
-                                        obs_b, obs_kind, obs_count, nullptr, (cudaStream_t)stream);
+                                        obs_b, obs_kind, obs_count, nullptr, nullptr, 0, nullptr, (cudaStream_t)stream);
 }
 
 int rda_convert_obstacles_ids(int B, int M, int N, int T, int E, float dt, int time_varying, int order,
@@ -857,10 +919,10 @@ int rda_convert_world_obstacles_ids(int B, int W, int N, int T, int E, float dt,
                                     const float* fleet_plan_xy, float* obs_A, float* obs_b, int32_t* obs_kind,
                                     int32_t* obs_count, int32_t* obs_id, void* stream) {
   if (!obs_id) return RDA_E_ARG;
-  return launch_world_obstacles(fleet_start != nullptr, B, W, N, T, E, dt, time_varying, order, state, world_start,
+  return launch_world_obstacles(fleet_start != nullptr, false, B, W, N, T, E, dt, time_varying, order, state, world_start,
                                 robot_world, shape_kind, shape_nv, shape_xy, shape_radius, shape_vel, fleet_start,
                                 fleet_robot, fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel, fleet_plan_xy,
-                                obs_A, obs_b, obs_kind, obs_count, obs_id, (cudaStream_t)stream);
+                                obs_A, obs_b, obs_kind, obs_count, obs_id, nullptr, 0, nullptr, (cudaStream_t)stream);
 }
 
 int rda_convert_world_obstacles_horizon_ids(int B, int W, int N, int T, int E, float dt, int time_varying,
@@ -876,11 +938,47 @@ int rda_convert_world_obstacles_horizon_ids(int B, int W, int N, int T, int E, f
                                             float* obs_b, int32_t* obs_kind, int32_t* obs_count, int32_t* obs_id,
                                             void* stream) {
   if (!obs_id) return RDA_E_ARG;
-  return launch_world_obstacles_horizon(B, W, N, T, E, dt, time_varying, nom_s, ref_s, body_kind, body_nv, body_xy,
+  return launch_world_obstacles_horizon(false, B, W, N, T, E, dt, time_varying, nom_s, ref_s, body_kind, body_nv, body_xy,
                                         body_radius, body_xy_b, body_radius_b, world_start, robot_world, shape_kind,
                                         shape_nv, shape_xy, shape_radius, shape_vel, fleet_start, fleet_robot,
                                         fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel, fleet_plan_xy, obs_A,
-                                        obs_b, obs_kind, obs_count, obs_id, (cudaStream_t)stream);
+                                        obs_b, obs_kind, obs_count, obs_id, nullptr, 0, nullptr, (cudaStream_t)stream);
+}
+
+int rda_convert_world_obstacles_traj(int B, int W, int N, int T, int E, float dt, int time_varying, int order,
+                                     const float* state, const int32_t* world_start, const int32_t* robot_world,
+                                     const int32_t* shape_kind, const int32_t* shape_nv, const float* shape_xy,
+                                     const float* shape_radius, const float* shape_vel, const int32_t* fleet_start,
+                                     const int32_t* fleet_robot, const int32_t* fleet_kind, const int32_t* fleet_nv,
+                                     const float* fleet_xy, const float* fleet_radius, const float* fleet_vel,
+                                     const float* fleet_plan_xy, float* obs_A, float* obs_b, int32_t* obs_kind,
+                                     int32_t* obs_count, int32_t* obs_id, const int32_t* shape_traj, int K,
+                                     const float* traj_xy, void* stream) {
+  return launch_world_obstacles(fleet_start != nullptr, true, B, W, N, T, E, dt, time_varying, order, state,
+                                world_start, robot_world, shape_kind, shape_nv, shape_xy, shape_radius, shape_vel,
+                                fleet_start, fleet_robot, fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel,
+                                fleet_plan_xy, obs_A, obs_b, obs_kind, obs_count, obs_id, shape_traj, K, traj_xy,
+                                (cudaStream_t)stream);
+}
+
+int rda_convert_world_obstacles_horizon_traj(int B, int W, int N, int T, int E, float dt, int time_varying,
+                                             const float* nom_s, const float* ref_s, int body_kind, int body_nv,
+                                             const float* body_xy, float body_radius, const float* body_xy_b,
+                                             const float* body_radius_b, const int32_t* world_start,
+                                             const int32_t* robot_world, const int32_t* shape_kind,
+                                             const int32_t* shape_nv, const float* shape_xy, const float* shape_radius,
+                                             const float* shape_vel, const int32_t* fleet_start,
+                                             const int32_t* fleet_robot, const int32_t* fleet_kind,
+                                             const int32_t* fleet_nv, const float* fleet_xy, const float* fleet_radius,
+                                             const float* fleet_vel, const float* fleet_plan_xy, float* obs_A,
+                                             float* obs_b, int32_t* obs_kind, int32_t* obs_count, int32_t* obs_id,
+                                             const int32_t* shape_traj, int K, const float* traj_xy, void* stream) {
+  return launch_world_obstacles_horizon(true, B, W, N, T, E, dt, time_varying, nom_s, ref_s, body_kind, body_nv,
+                                        body_xy, body_radius, body_xy_b, body_radius_b, world_start, robot_world,
+                                        shape_kind, shape_nv, shape_xy, shape_radius, shape_vel, fleet_start,
+                                        fleet_robot, fleet_kind, fleet_nv, fleet_xy, fleet_radius, fleet_vel,
+                                        fleet_plan_xy, obs_A, obs_b, obs_kind, obs_count, obs_id, shape_traj, K,
+                                        traj_xy, (cudaStream_t)stream);
 }
 
 int rda_post_process(int B, int T, int P, int goal_index_threshold, const int32_t* near_index, float* u_opt,

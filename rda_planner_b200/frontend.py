@@ -115,6 +115,35 @@ def _pack_shape(out, at, o, max_edge_num):
         out['xy'][at + (slice(0, n),)] = v[0:2].T
 
 
+def _pack_trajectory(o, max_edge_num):
+    """The trajectory of one simulator obstacle -> float32 [T+1, 8, 2], its shape at every stage in the world frame: a
+    polygon's vertices (T+1 arrays 2 x nv, nv that of its vertex), a disc's centre in row 0 (centres 2 x (T+1))."""
+    xy = None
+    if o.cone_type == 'norm2':
+        c = np.asarray(o.trajectory, float)
+        if c.ndim != 2 or c.shape[0] != 2 or c.shape[1] < 1:
+            raise ValueError(f'a disc trajectory is 2 x (T+1) centres, got shape {c.shape}')
+        xy = np.zeros((c.shape[1], _cabi.MAX_EDGE, 2))
+        xy[:, 0] = c.T
+    else:
+        nv = np.asarray(o.vertex).shape[1]
+        stages = [np.asarray(v, float) for v in o.trajectory]
+        if not stages:
+            raise ValueError('a polygon trajectory has at least one stage')
+        for t, v in enumerate(stages):
+            if v.ndim != 2 or v.shape[0] < 2 or v.shape[1] != nv:
+                raise ValueError(f'stage {t} of a polygon trajectory has shape {v.shape}: 2 x {nv} vertices, as its '
+                                 'vertex, at every stage')
+        if nv > min(max_edge_num, _cabi.MAX_EDGE):
+            raise ValueError(f'polygon trajectory with {nv} vertices: 3..{min(max_edge_num, _cabi.MAX_EDGE)} supported')
+        xy = np.zeros((len(stages), _cabi.MAX_EDGE, 2))
+        for t, v in enumerate(stages):
+            xy[t, :nv] = v[0:2].T
+    if not np.all(np.isfinite(xy)):
+        raise ValueError('a trajectory has non-finite values')
+    return xy.astype(np.float32)
+
+
 def pack_shapes(obstacle_lists, max_shapes=None, max_edge_num=_cabi.MAX_EDGE):
     """Per-instance lists of simulator obstacles (attributes cone_type, center, radius, vertex,
     velocity — what MPC.convert_rda_obstacle reads, mpc.py:189-208) -> dict of host arrays in
@@ -131,6 +160,9 @@ def pack_shapes(obstacle_lists, max_shapes=None, max_edge_num=_cabi.MAX_EDGE):
             raise ValueError('more obstacles than max_shapes')
         out['count'][b] = len(lst)
         for j, o in enumerate(lst):
+            if getattr(o, 'trajectory', None) is not None:
+                raise ValueError('obstacles with a trajectory are packed by pack_worlds (one world per robot, '
+                                 'robot_world = arange(B), gives per-robot lists)')
             _pack_shape(out, (b, j), o, max_edge_num)
     return out
 
@@ -139,7 +171,15 @@ def pack_worlds(worlds, max_edge_num=_cabi.MAX_EDGE):
     """W lists of simulator obstacles (as pack_shapes takes them), each shared by any number of robots, of any
     size -> dict of host arrays in the layout of rda_convert_world_obstacles: kind, nv, xy, radius, vel over the
     flat list of all worlds' shapes, and start [W+1] (world w is shapes start[w]:start[w+1]).  The shape arrays
-    have at least one entry, so that a set of empty worlds still has device buffers to point at."""
+    have at least one entry, so that a set of empty worlds still has device buffers to point at.
+
+    An obstacle may carry a `trajectory`, its predicted shape at every stage t = 0..T in the world frame: for a polygon
+    T+1 vertex arrays 2 x nv (nv that of its vertex), for a disc the centres 2 x (T+1).  When one does, the dict also
+    holds traj [S] int32 (each shape's trajectory, -1 for none) and traj_xy [K, T+1, 8, 2] float32 (trajectory k's
+    stage-t vertices, or a disc's centre in row 0), the table of rda_convert_world_obstacles_traj; xy then holds stage 0
+    and vel zero for the shapes with a trajectory.  Both may be overwritten on the device between control steps (a
+    predictor's output) without packing again: keep the shape, the dtype and the storage.  Without trajectories the
+    dict is exactly what it was."""
     sizes = [len(l) for l in worlds]
     if not sizes:
         raise ValueError('at least one world')
@@ -148,11 +188,51 @@ def pack_worlds(worlds, max_edge_num=_cabi.MAX_EDGE):
     if start[-1] > np.iinfo(np.int32).max:
         raise ValueError('more than 2**31 - 1 shapes')
     out = _shape_arrays(max(1, int(start[-1])))
+    trajs = []
     for w, lst in enumerate(worlds):
         for j, o in enumerate(lst):
             _pack_shape(out, (int(start[w]) + j,), o, max_edge_num)
+            if getattr(o, 'trajectory', None) is not None:
+                trajs.append((int(start[w]) + j, _pack_trajectory(o, max_edge_num)))
     out['start'] = start.astype(np.int32)
+    if trajs:
+        stages = {len(xy) for _, xy in trajs}
+        if len(stages) != 1:
+            raise ValueError(f'trajectories of different stage counts {sorted(stages)}: every one has T+1 stages')
+        out['traj'] = np.full(len(out['kind']), -1, np.int32)
+        out['traj_xy'] = np.stack([xy for _, xy in trajs])
+        for k, (at, xy) in enumerate(trajs):
+            out['traj'][at] = k
+            out['xy'][at] = xy[0]
+            out['vel'][at] = 0
     return out
+
+
+def _check_traj(world, T, time_varying, device=None):
+    """Refuse, with a ValueError, a world with trajectories (pack_worlds) that a call with horizon T and time_varying
+    cannot take: time-invariant output, traj_xy not [K, T+1, 8, 2], and with `device` (the conversions) traj_xy /
+    traj that are not contiguous float32 / int32 [S] tensors on that device."""
+    if not time_varying:
+        raise ValueError('a world with trajectories needs time_varying=True: a trajectory is T+1 copies')
+    txy, traj = world['traj_xy'], world['traj']
+    if len(txy.shape) != 4 or txy.shape[1] != T + 1:
+        raise ValueError(f"world['traj_xy'] has shape {tuple(txy.shape)}: [K, T+1, 8, 2] with T+1 = {T + 1} stages")
+    if tuple(txy.shape[2:]) != (_cabi.MAX_EDGE, 2) or txy.shape[0] < 1:
+        raise ValueError(f"world['traj_xy'] has shape {tuple(txy.shape)}: [K, T+1, {_cabi.MAX_EDGE}, 2], K >= 1")
+    if tuple(traj.shape) != tuple(world['kind'].shape):
+        raise ValueError(f"world['traj'] has shape {tuple(traj.shape)}: one entry per packed shape, "
+                         f"{tuple(world['kind'].shape)}")
+    if device is None:
+        return
+    for name, t, dtype in (('traj_xy', txy, torch.float32), ('traj', traj, torch.int32)):
+        if not isinstance(t, torch.Tensor) or t.dtype != dtype or t.device != device or not t.is_contiguous():
+            raise ValueError(f"world['{name}'] must be a contiguous {dtype} tensor on {device}")
+
+
+def _traj_args(world, T, time_varying, device):
+    """(shape_traj, K, traj_xy) of a world with trajectories, checked against the call (_check_traj)."""
+    _check_traj(world, T, time_varying, device)
+    return _ptr(world['traj']), world['traj_xy'].shape[0], _ptr(world['traj_xy'])
 
 
 def pre_process_batch(state, cur_vel, ref_speed, path, start_index, dynamics, dt, wheelbase, T,
@@ -203,7 +283,8 @@ def convert_world_obstacles_batch(world, state, robot_world, N, T, E, dt, time_v
     shapes of its world (order) or its first N, as convert_obstacles_batch would given the whole world as its
     list.  Returns obs_A [B,N,Tc,E,2], obs_b [B,N,Tc,E], obs_kind [B,N], obs_count [B] (the world sizes), and with ids
     also obs_id [B,N] int32: the flat index of each slot's shape in the packed worlds (-1 for an empty world), for
-    RDA_solver.set_obstacle_ids."""
+    RDA_solver.set_obstacle_ids.  A world with trajectories (traj, traj_xy) needs time_varying: its shapes are keyed
+    by their stage 0 and written along their trajectories (rda_convert_world_obstacles_traj)."""
     lib = _cabi.load()
     dev = state.device
     B, W = state.shape[0], world['start'].shape[0] - 1
@@ -212,6 +293,16 @@ def convert_world_obstacles_batch(world, state, robot_world, N, T, E, dt, time_v
     b = torch.empty((B, N, Tc, E), dtype=torch.float32, device=dev)
     kind = torch.empty((B, N), dtype=torch.int32, device=dev)
     count = torch.empty(B, dtype=torch.int32, device=dev)
+    if 'traj' in world:
+        traj = _traj_args(world, T, time_varying, dev)
+        obs_id = torch.empty((B, N), dtype=torch.int32, device=dev) if ids else None
+        with torch.cuda.device(dev):
+            _cabi.check(lib.rda_convert_world_obstacles_traj(
+                B, W, N, T, E, dt, int(time_varying), int(order), _ptr(state), _ptr(world['start']), _ptr(robot_world),
+                _ptr(world['kind']), _ptr(world['nv']), _ptr(world['xy']), _ptr(world['radius']), _ptr(world['vel']),
+                *(None,) * 8, _ptr(A), _ptr(b), _ptr(kind), _ptr(count), _ptr(obs_id), *traj, _stream(dev)),
+                'rda_convert_world_obstacles_traj')
+        return (A, b, kind, count, obs_id) if ids else (A, b, kind, count)
     if ids:
         obs_id = torch.empty((B, N), dtype=torch.int32, device=dev)
         with torch.cuda.device(dev):
@@ -321,7 +412,8 @@ def convert_fleet_obstacles_batch(world, state, robot_world, fleet, N, T, E, dt,
     size plus the robots of the world minus one).  plan: the stage-t copy of a mate is its body along its plan,
     fleet['plan_xy'][m, t] (from fleet_plan_shapes_batch), instead of its shape moved at constant velocity; the same
     slots in the same order.  Needs time_varying.  ids: also returns obs_id [B,N] int32, each slot's obstacle: the flat
-    index of a world shape, S + m for map-mate robot m (S the number of packed shapes), -1 for an empty list."""
+    index of a world shape, S + m for map-mate robot m (S the number of packed shapes), -1 for an empty list.  A world
+    with trajectories: as convert_world_obstacles_batch."""
     if plan and not time_varying:
         raise ValueError('a fleet predicted along its plans needs time_varying=True')
     lib = _cabi.load()
@@ -338,6 +430,14 @@ def convert_fleet_obstacles_batch(world, state, robot_world, fleet, N, T, E, dt,
             _ptr(csr[0]), _ptr(csr[1]), _ptr(fleet['kind']), _ptr(fleet['nv']), _ptr(fleet['xy']), _ptr(fleet['radius']),
             _ptr(fleet['vel']))
     outs = (_ptr(A), _ptr(b), _ptr(kind), _ptr(count), _stream(dev))
+    if 'traj' in world:
+        traj = _traj_args(world, T, time_varying, dev)
+        obs_id = torch.empty((B, N), dtype=torch.int32, device=dev) if ids else None
+        with torch.cuda.device(dev):
+            _cabi.check(lib.rda_convert_world_obstacles_traj(*args, _ptr(fleet['plan_xy']) if plan else None,
+                                                             *outs[:4], _ptr(obs_id), *traj, outs[4]),
+                        'rda_convert_world_obstacles_traj')
+        return (A, b, kind, count, obs_id) if ids else (A, b, kind, count)
     with torch.cuda.device(dev):
         if ids:
             obs_id = torch.empty((B, N), dtype=torch.int32, device=dev)
@@ -360,7 +460,8 @@ def convert_world_obstacles_horizon_batch(world, nom_s, ref_s, body, robot_world
     body from robot_body with xy a CUDA tensor; per_robot None, or a dict with CUDA tensors 'xy' [B,8,2] and 'radius'
     [B], each robot's own body (body gives the kind and vertex count).  The same list, padding, outputs and obs_count
     as those calls; without a host synchronisation.  ids: also returns obs_id [B,N] int32, the ids of
-    convert_fleet_obstacles_batch."""
+    convert_fleet_obstacles_batch.  A world with trajectories: as convert_world_obstacles_batch, the horizon key taken
+    over each trajectory's stage-t rows."""
     if plan and (fleet is None or not time_varying):
         raise ValueError('a fleet predicted along its plans needs a fleet and time_varying=True')
     lib = _cabi.load()
@@ -381,6 +482,13 @@ def convert_world_obstacles_horizon_batch(world, nom_s, ref_s, body, robot_world
             _ptr(body['xy']), float(body['radius']), _ptr(pr.get('xy')), _ptr(pr.get('radius')), _ptr(world['start']),
             _ptr(robot_world), _ptr(world['kind']), _ptr(world['nv']), _ptr(world['xy']), _ptr(world['radius']),
             _ptr(world['vel']), *mates, _ptr(A), _ptr(b), _ptr(kind), _ptr(count))
+    if 'traj' in world:
+        traj = _traj_args(world, T, time_varying, dev)
+        obs_id = torch.empty((B, N), dtype=torch.int32, device=dev) if ids else None
+        with torch.cuda.device(dev):
+            _cabi.check(lib.rda_convert_world_obstacles_horizon_traj(*args, _ptr(obs_id), *traj, _stream(dev)),
+                        'rda_convert_world_obstacles_horizon_traj')
+        return (A, b, kind, count, obs_id) if ids else (A, b, kind, count)
     with torch.cuda.device(dev):
         if ids:
             obs_id = torch.empty((B, N), dtype=torch.int32, device=dev)
@@ -432,7 +540,12 @@ class BatchedMPC:
     (RDA_solver.set_obstacle_ids), and info['obs_id'] [B,N] says which obstacle each slot held.  An obstacle's identity
     is its list position: its flat index in the packed world (pack_worlds), S + m for map-mate robot m (S packed shapes),
     its position in a robot's shapes= list.  A caller who repacks a map must keep its order for the warm start to
-    follow.  A step without obstacles gives every slot the id -1, so each slot starts cold when obstacles come back."""
+    follow.  A step without obstacles gives every slot the id -1, so each slot starts cold when obstacles come back.
+
+    A world from pack_worlds whose obstacles carry trajectories (traj, traj_xy) makes those shapes follow them over the
+    horizon, the reference's time-varying rdaobs (MPC(rda_obstacle=True)): keyed by their stage 0, written along their
+    stages, with every obstacle_order, avoid_fleet, fleet_prediction and warm_start, and time_varying=True.  The caller
+    may overwrite world['traj_xy'] (and world['traj']) on the device between steps, e.g. with a predictor's output."""
 
     def __init__(self, car_tuple, ref_path, batch, receding=10, sample_time=0.1, iter_num=4,
                  enable_reverse=False, obstacle_order=True, max_edge_num=5, max_obs_num=5,
@@ -588,6 +701,11 @@ class BatchedMPC:
                 if self._no_world is None:
                     self._no_world = shapes_to_device(pack_worlds([[]]), dev)
                 world = self._no_world
+        if shapes is not None and 'traj' in shapes:
+            raise ValueError('obstacles with trajectories are selected from worlds, not from shapes=: pass the lists as '
+                             'worlds (world=pack_worlds(lists), one world per robot, robot_world=arange(B))')
+        if world is not None and 'traj' in world:
+            _check_traj(world, T, time_varying)
         if world is not None:
             if shapes is not None:
                 raise ValueError('pass either shapes or world, not both')
