@@ -26,6 +26,8 @@ ROUTING_ENV = {                     # environment read by rda_create
     'stream': {'RDA_B200_SMALL': '0'},
     'extra': {'RDA_B200_SMALL': '0', 'RDA_B200_EXTRA_MIN': '1'},
     'split': {'RDA_B200_SMALL': '0', 'RDA_B200_SPLIT_MIN': '2', 'RDA_B200_SPLIT_PARTS': '2'},
+    'split3': {'RDA_B200_SMALL': '0', 'RDA_B200_SPLIT_MIN': '2', 'RDA_B200_SPLIT_PARTS': '3'},
+    'coherent': {'RDA_B200_SMALL': '0', 'RDA_B200_LEAN2': '1'},     # polygon body, E <= 4: k_cells_coh first
 }
 KNOBS = ('RDA_B200_SMALL', 'RDA_B200_LEAN2', 'RDA_B200_EXTRA_MIN', 'RDA_B200_SMALL_BULK', 'RDA_B200_SPLIT_MIN',
          'RDA_B200_SPLIT_PARTS')
@@ -92,19 +94,28 @@ CELL_CASES += [(E, 'disc', 'stream') for E in (3, 5, 8)]
 
 @pytest.mark.parametrize('E,body,routing', CELL_CASES)
 def test_every_cell_equals_generic_solver(monkeypatch, E, body, routing):
+    """Every cell of the second cell step of a batch of B = 4, T = 8, N = 4 against the float64 generic solver
+    (check_every_cell)."""
+    B, T, N = 4, 8, 4
+    car = _car(body)
+    disc = body == 'disc'
+    # the disc body is narrower than the rectangle: a closer band gives it active cells, which the searched passes take
+    inp = _batch(car, B, T, N, E, 9300 + 10 * E, lateral=(0.0, 1.2) if disc else (0.2, 2.5))
+    cnt = check_every_cell(monkeypatch, routing, car, disc, inp, T, N, E, f'E = {E}, {body}')
+    assert cnt[2] == 0 and cnt[1] > 0                   # the searched passes saw cells of this layout
+
+
+def check_every_cell(monkeypatch, routing, car, disc, inp, T, N, E, label):
     """Phase API, two ADMM iterations.  Every cell of the second cell step against solve_cell_generic in float64 on the float32
     inputs the kernels read: lam (E rows), mu (R rows), z, zeta_new, xi_new = xi + Hm, the su-QP coefficients rebuilt by
     DESIGN.md §2 (a = lam'A, c0 relative to pref, g = mu'G + xi_new), and the per-instance residuals of finish() against their
     float64 recomputation from the kernels' own multipliers.  Tolerances of test_gpu_robot_bodies.py; lam compared as in
-    test_cells_many_edges.py (row scale, flat vertices, the float32 tolerance grown below FLAT)."""
-    B, T, N, ro2 = 4, 8, 4, 1.0
-    car = _car(body)
-    disc = body == 'disc'
+    test_cells_many_edges.py (row scale, flat vertices, the float32 tolerance grown below FLAT).  Returns the cell counters
+    of the two cell steps (fast, searched, failed, ...)."""
+    B, ro2 = len(inp['nom_s']), 1.0
     G, h = (np.asarray(car.G, float), np.asarray(car.h, float)) if disc else canonical_polygon_rows(car.G, car.h)
     h = np.asarray(h).ravel()
     R = G.shape[0]
-    # the disc body is narrower than the rectangle: a closer band gives it active cells, which the searched passes take
-    inp = _batch(car, B, T, N, E, 9300 + 10 * E, lateral=(0.0, 1.2) if disc else (0.2, 2.5))
     g = _solver(monkeypatch, routing, car, T, N, E, 2, B)
     g.begin(**_cuda(inp), time_varying=False, iter_threshold=0.0)
     g.step_su(); g.step_lammuz()
@@ -178,10 +189,10 @@ def test_every_cell_equals_generic_solver(monkeypatch, E, body, routing):
         assert abs(out['resi_pri'][bi] - np.sqrt(hm2)) <= 1e-3 * (1 + np.sqrt(hm2)), (bi, out['resi_pri'][bi], np.sqrt(hm2))
         assert abs(out['resi_dual'][bi] - dual / N) <= 1e-3 * (1 + dual / N), (bi, out['resi_dual'][bi], dual / N)
     cnt = after['COUNTERS'].astype(int)
-    print(f'\nE = {E}, {body} (R = {R}), {routing}: largest gap to the float64 reference {worst}; {B * N * T} cells, {active} '
+    print(f'\n{label} (R = {R}), {routing}: largest gap to the float64 reference {worst}; {B * N * T} cells, {active} '
           f'active, {refereed} refereed, obstacles with a vertex flatter than {FLAT}: {flat}; cells per pass fast / searched / '
           f'failed {cnt[:3].tolist()}, launches of the cell step {launches}')
-    assert cnt[2] == 0 and cnt[1] > 0                   # the searched passes saw cells of this layout
+    return cnt
 
 
 def test_config_d_shape_every_cell_feasible(monkeypatch):

@@ -43,8 +43,12 @@ def _slot_view(x, kind, B, N, T, E, R):
 
 @pytest.mark.parametrize('N,E,disc', [(5, 4, False), (20, 4, False), (7, 8, True), (256, 3, False), (300, 3, False)])
 def test_remap_kernel_is_the_numpy_rule_bit_for_bit(N, E, disc):
-    rng = np.random.default_rng(N + E)
-    B, T = 48, 6
+    check_remap_kernel(48, 6, N, E, disc, N + E)
+
+
+def check_remap_kernel(B, T, N, E, disc, seed):
+    """k_remap_slots on random slot states and random id lists against the numpy rule of obstacle_ids_twin, bit for bit."""
+    rng = np.random.default_rng(seed)
     car = disc_robot() if disc else rectangle_robot()
     g = RDA_solver(T, car, max_edge_num=E, max_obs_num=N, iter_num=1, time_print=False, batch=B, device=DEV)
     R = 3 if disc else 4
